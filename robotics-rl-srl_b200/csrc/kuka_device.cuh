@@ -54,6 +54,17 @@
 #define KK_PROBE_D(d)
 #define KK_PROBE_SWEEP()
 #endif
+// Diagnostic build (scripts/build_variant.sh phases -DKK_PHASES, scripts/kuka_phase_timing.py): clock64() accumulators per phase of the
+// micro-step loop, in registers, stored per env slot at the end of the launch.  Separate from KK_TIMING, whose convergence probe adds
+// instructions to every sweep row.  KK_PH(clk, k) charges the cycles since the previous mark to phase k; without KK_PHASES it is empty.
+enum { KK_PH_KIN = 0, KK_PH_IK, KK_PH_DYN, KK_PH_CHOL, KK_PH_SETUP, KK_PH_FAST, KK_PH_GENERAL, KK_PH_ENV, KK_NPH };
+#if defined(KK_PHASES) && defined(__CUDACC__)
+struct KkPhaseClock { long long last; long long acc[KK_NPH]; };
+#define KK_PH(clk, k) do { if (clk) { const long long t_ = clock64(); (clk)->acc[k] += t_ - (clk)->last; (clk)->last = t_; } } while (0)
+#else
+struct KkPhaseClock { long long dummy; };
+#define KK_PH(clk, k) do { (void)(clk); } while (0)
+#endif
 struct f3 { float x, y, z; };
 struct alignas(16) kk_f4 { float x, y, z, w; };   // one 128-bit load (host-compilable stand-in for float4)
 KK_DEV f3 mk3(float x, float y, float z) { f3 r; r.x = x; r.y = y; r.z = z; return r; }
@@ -674,7 +685,8 @@ KK_DEV void kuka_spd_inverse(float (&M)[KK_NB][KK_NB]) {
 struct KkNoScratch { float dummy; KK_DEV float& operator[](int) const { return const_cast<float&>(dummy); } };
 template <bool JOINTS, bool TWOB, bool COOP = false, class SC = KkNoScratch>
 KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k, const KukaContacts& ct, bool button_armed, const float* q_joints,
-                              const SC& sc = SC(), int u = 0, unsigned gmask = 0u, int nc_coop = 0, unsigned* dbg = nullptr) {
+                              const SC& sc = SC(), int u = 0, unsigned gmask = 0u, int nc_coop = 0, unsigned* dbg = nullptr,
+                              KkPhaseClock* ph = nullptr) {
     constexpr int ND = TWOB ? KK_NB + 2 : KK_NB + 1;
     // ---- applyAction: IK + motor set-points (kuka.py:142-187) ----
     float q_ik[7];
@@ -692,6 +704,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         for (int t = 0; t < 9; ++t) kk7.R6[t] = sc[6 * KC_BS + KB_R + t];
         kuka_ik(P, e, kk7, q_ik);
     } else kuka_ik(P, e, k, q_ik);
+    KK_PH(ph, KK_PH_IK);
     // ---- dynamics ----
     float A[KK_NB][KK_NB], bias[KK_NB];
     if constexpr (COOP) {
@@ -705,9 +718,11 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
 #pragma unroll
             for (int j = 0; j <= i; ++j) A[i][j] = sc[KC_OFF_MA + i * KC_MS + j];
         }
+        KK_PH(ph, KK_PH_DYN);
         // Cholesky + M^-1 in registers, by every lane: dealt to the 4 lanes through shared memory it was three times slower (12 dependent
         // pivot steps of load -> rsqrt -> scale -> store -> barrier)
         kuka_spd_inverse(A);
+        KK_PH(ph, KK_PH_CHOL);
     } else {
 #if KK_ROLL_DYN
     {
@@ -723,7 +738,9 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
 #else
     kuka_dynamics(P, e, k, A, bias);
 #endif
+    KK_PH(ph, KK_PH_DYN);
     kuka_spd_inverse(A);
+    KK_PH(ph, KK_PH_CHOL);
     }
     float v[ND];
     {
@@ -914,6 +931,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
     bool kk_probe_any = false; int kk_probe_sweep = 0, kk_probe_conv = 0;
 #endif
     bool resume_mid_sweep = false;  // the fast loop already ran the motor + button rows of sweep it0
+    KK_PH(ph, KK_PH_SETUP);
     if ((lim_lo_mask | lim_hi_mask) == 0u) {
         // FAST LOOP (no arm joint on a limit): straight-line sweep, registers only.  Contact rows of the manifold are
         // WATCHED: while every normal row is separating (lam = 0 and J v >= target) it and its friction rows are exact
@@ -1029,6 +1047,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         if (dbg && nc > 0) *dbg |= 1u;
 #endif
     }
+    KK_PH(ph, KK_PH_FAST);
 #ifdef KK_TIMING
     if (dbg) *dbg |= ((unsigned)kk_probe_conv & 255u) << 24;
     if (dbg) { *dbg |= ((unsigned)nc & 15u) << 2; if (lim_lo_mask | lim_hi_mask) *dbg |= 64u; if (it0 < P.iters) *dbg |= 2u | ((unsigned)(P.iters - it0) & 255u) << 8; }
@@ -1096,6 +1115,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
             }
         }
     }
+    KK_PH(ph, KK_PH_GENERAL);
 #undef KK_MOTOR_ROWS
 #undef KK_MOTOR_ROWS_WATCH
 #undef KK_ROW_PTR
@@ -1109,4 +1129,5 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
     for (int i = 0; i < KK_NB; ++i) { e.qd[i] = v[i]; e.q[i] = fmaf(P.dt, v[i], e.q[i]); }
     e.qdb = v[KK_NB]; e.qb = fmaf(P.dt, v[KK_NB], e.qb);
     if (TWOB) { e.qdb2 = v[ND - 1]; e.qb2 = fmaf(P.dt, v[ND - 1], e.qb2); }
+    KK_PH(ph, KK_PH_SETUP);
 }

@@ -222,6 +222,11 @@ __device__ unsigned long long kk_timing[1 << 16];
 #else
 #define KK_TIMING_RECORD() do { } while (0)
 #endif
+#ifdef KK_PHASES
+// diagnostic build (scripts/build_variant.sh phases -DKK_PHASES): per env slot of the LAST launch, cycles spent in each phase of the micro-step
+// loop (KK_PH_* of kuka_device.cuh), then the number of physics steps the slot ran
+__device__ unsigned long long kk_phase[1 << 13][KK_NPH + 1];
+#endif
 template <bool JOINTS, bool TWOB, bool PREFETCH = false, bool COOP = false>
 __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ KukaDev d, int n, int op, int T,
                                                        const void* __restrict__ actions, const float* __restrict__ noise,
@@ -235,6 +240,14 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
     const int lane = threadIdx.x & 31, warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
 #ifdef KK_TIMING
     const long long kk_t0 = clock64(); unsigned dbgf = 0u;
+#endif
+#ifdef KK_PHASES
+    KkPhaseClock kk_ph_clk; KkPhaseClock* const ph = &kk_ph_clk; unsigned kk_nphys = 0u;
+    kk_ph_clk.last = clock64();
+#pragma unroll
+    for (int k2 = 0; k2 < KK_NPH; ++k2) kk_ph_clk.acc[k2] = 0;
+#else
+    KkPhaseClock* const ph = nullptr;
 #endif
     const int slot = COOP ? lane >> 2 : lane;            // env slot within the warp
     const int u = COOP ? lane & 3 : 0;
@@ -324,13 +337,55 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
             }
         }
     }
+    // COOP: an env that is done with the loop does not leave it alone: it waits at the loop head until every env of its warp is done.
+    // The vote there is the one point where all groups of the warp meet at the start of every micro-step.  Without it, a group that
+    // branches off (reset(), a taken record, the end of the rollout) stays off the others' instruction stream for the rest of the launch:
+    // a group running its reset micro-steps and the groups running their env steps execute the same code at different times, and the warp
+    // issues every instruction of the sweeps once per stream.  (Lanes that returned before the loop have exited, which the vote allows.)
+    // what an env does when it leaves the micro-step loop: write its state back (or publish its next-episode record).  With 4 lanes per env
+    // this runs where the env leaves, before it waits for the rest of its warp: a record completed by a helper slot is published while the
+    // other envs of the launch are still running, so an episode that ends later in the same launch can take it
+    auto leave = [&]() {
+        e.cbutton = saved_cb; e.ctable = saved_ct;
+        if (TWOB) { e.cany0 = saved_a0; e.cany1 = saved_a1; }
+        KK_TIMING_RECORD();
+#ifdef KK_PHASES
+        KK_PH(ph, KK_PH_ENV);
+        if (lead) {
+            unsigned long long* const kp = kk_phase[(warp * (COOP ? 8 : 32) + slot) & ((1 << 13) - 1)];
+#pragma unroll
+            for (int k2 = 0; k2 < KK_NPH; ++k2) kp[k2] = (unsigned long long)kk_ph_clk.acc[k2];
+            kp[KK_NPH] = kk_nphys;
+        }
+#endif
+        if constexpr (PREFETCH) {
+            if (op == KUKA_OP_PREFETCH) {
+                if (!lead) return;
+                env_store<TWOB>(nx, i, e);
+                if (partial) { nx.progress[i] = (uint8_t)(N_RANDOM_ACTIONS_AT_INIT - reset_left); return; }   // nx.episode[i] was set when the record was begun
+                nx.episode[i] = (int)e.episode - 1;   // record first, then the episode it is for, then the flag
+                nx.progress[i] = 0;
+                __threadfence();
+                reinterpret_cast<volatile uint8_t*>(nx.valid)[i] = 1;
+                return;
+            }
+        }
+        if (lead) env_store<TWOB>(d, i, e);
+    };
+    bool fin = false, settled = false;
+#define KK_LEAVE_LOOP() { if (COOP) { leave(); fin = true; continue; } else break; }
     for (;;) {
+        if constexpr (COOP) {
+            if (__all_sync(0xffffffffu, fin)) break;
+            if (fin) continue;
+        }
         // link states of the configuration just reached + collision detection for the next step
         if constexpr (COOP) {
             KcKinIn kin;
 #pragma unroll
             for (int j = 0; j < KK_NB; ++j) kin.q[j] = e.q[j];
             kin.qb = e.qb; kin.qb2 = e.qb2; kin.bbx = e.bbx; kin.bby = e.bby; kin.bbz = e.bbz; kin.bb2x = e.bb2x; kin.bb2y = e.bb2y;
+            KK_PH(ph, KK_PH_ENV);
             __syncwarp(gmask);   // the group is done with the rows / matrices of the previous micro-step (the candidates reuse that storage)
             const bool near = kc_kinematics<TWOB>(sc, kc_tab, P, kin, u, gmask);
             e.grip[0] = sc[8 * KC_BS + KB_C]; e.grip[1] = sc[8 * KC_BS + KB_C + 1]; e.grip[2] = sc[8 * KC_BS + KB_C + 2];   // getLinkState(kuka, 8)[0]: COM of link 8
@@ -339,7 +394,8 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
             e.cbutton = fl & 1; e.ctable = (fl >> 1) & 1;
             if (TWOB) { e.cany0 = (fl >> 2) & 1; e.cany1 = (fl >> 3) & 1; }
             nc_reg = near ? (int)sc[KC_OFF_LINK + 7] : 0;
-        } else kuka_fk<true, TWOB>(P, e, k, ct);
+            KK_PH(ph, KK_PH_KIN);
+        } else { KK_PH(ph, KK_PH_ENV); kuka_fk<true, TWOB>(P, e, k, ct); KK_PH(ph, KK_PH_KIN); }
         const int new_cb = e.cbutton, new_ct = e.ctable, new_a0 = TWOB ? e.cany0 : 0, new_a1 = TWOB ? e.cany1 : 0;
         if (pending) {
             // ---- _reward() (:428-463): manifold of the step that just ran, link states after it ----
@@ -436,7 +492,8 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
                     for (int j = 0; j < KK_NB; ++j) { snap[j] = e.q[j]; snap[KK_NB + j] = e.qd[j]; }
                     snap[24] = e.ee[0]; snap[25] = e.ee[1]; snap[26] = e.ee[2]; snap[27] = e.qb; snap[28] = e.qdb;
                 }
-                return;
+                settled = true;                 // no state to write back
+                if (COOP) { fin = true; continue; } else break;
             }
             if (!(PREFETCH && consumed)) reset_end<TWOB>(P, e);
             consumed = false;
@@ -446,7 +503,7 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
             }
             if (op == KUKA_OP_ROLLOUT) ++t;
         }
-        if (!in_reset && (op != KUKA_OP_ROLLOUT || t >= T)) break;
+        if (!in_reset && (op != KUKA_OP_ROLLOUT || t >= T)) KK_LEAVE_LOOP()
         // ---- next micro action ----
         bool armed;
         if (in_reset) {
@@ -527,34 +584,25 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
         // ---- applyAction + stepSimulation ----
         if (!JOINTS) apply_ee_delta(P, e, dx, dy, dz);
         saved_cb = new_cb; saved_ct = new_ct; saved_a0 = new_a0; saved_a1 = new_a1;
-#ifdef KK_TIMING
-        kuka_physics_step<JOINTS, TWOB, COOP>(P, e, k, ct, armed, qj, sc, u, gmask, nc_reg, &dbgf);
-#else
-        kuka_physics_step<JOINTS, TWOB, COOP>(P, e, k, ct, armed, qj, sc, u, gmask, nc_reg);
+        KK_PH(ph, KK_PH_ENV);
+#ifdef KK_PHASES
+        ++kk_nphys;
 #endif
-        if constexpr (PREFETCH) { if (helper && --budget <= 0 && reset_left > 0) { partial = true; break; } }
+#ifdef KK_TIMING
+        kuka_physics_step<JOINTS, TWOB, COOP>(P, e, k, ct, armed, qj, sc, u, gmask, nc_reg, &dbgf, ph);
+#else
+        kuka_physics_step<JOINTS, TWOB, COOP>(P, e, k, ct, armed, qj, sc, u, gmask, nc_reg, nullptr, ph);
+#endif
+        if constexpr (PREFETCH) { if (helper && --budget <= 0 && reset_left > 0) { partial = true; KK_LEAVE_LOOP() } }
         if (!in_reset) {
             // step2()'s repeat loop (:349-354): stop repeating once terminated / past the step limit
             if (e.terminated || e.counter > P.max_steps) { pending = true; rep = 0; }
             else { e.counter += 1; if (++rep == P.action_repeat) { pending = true; rep = 0; } }
         }
     }
-    e.cbutton = saved_cb; e.ctable = saved_ct;
-    if (TWOB) { e.cany0 = saved_a0; e.cany1 = saved_a1; }
-    KK_TIMING_RECORD();
-    if constexpr (PREFETCH) {
-        if (op == KUKA_OP_PREFETCH) {
-            if (!lead) return;
-            env_store<TWOB>(nx, i, e);
-            if (partial) { nx.progress[i] = (uint8_t)(N_RANDOM_ACTIONS_AT_INIT - reset_left); return; }   // nx.episode[i] was set when the record was begun
-            nx.episode[i] = (int)e.episode - 1;   // record first, then the episode it is for, then the flag
-            nx.progress[i] = 0;
-            __threadfence();
-            reinterpret_cast<volatile uint8_t*>(nx.valid)[i] = 1;
-            return;
-        }
-    }
-    if (lead) env_store<TWOB>(d, i, e);
+#undef KK_LEAVE_LOOP
+    if (settled) return;
+    if constexpr (!COOP) leave();
 }
 
 // Scene primitives of every env for srl_sim_render (render_core.h): one thread per env recomputes the joint frames of the stored
@@ -962,6 +1010,12 @@ int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
 #ifdef KK_TIMING
     case 99: {   // diagnostic build: the per-slot timing words of the last launch
         if (cudaMemcpyFromSymbol(dst, kk_timing, bytes < sizeof(kk_timing) ? bytes : sizeof(kk_timing)) != cudaSuccess) return 1;
+        return 0;
+    }
+#endif
+#ifdef KK_PHASES
+    case 98: {   // diagnostic build: the per-slot phase cycles of the last launch, [slot][KK_NPH + 1]
+        if (cudaMemcpyFromSymbol(dst, kk_phase, bytes < sizeof(kk_phase) ? bytes : sizeof(kk_phase)) != cudaSuccess) return 1;
         return 0;
     }
 #endif

@@ -1,0 +1,78 @@
+"""Where the time of the fused Kuka rollout goes, phase by phase.  Needs the -DKK_PHASES build (scripts/build_variant.sh phases -DKK_PHASES,
+then SRL_SIM_CUDA_LIB=robotics-rl-srl_b200/csrc/libsrl_variant_phases.so): every env slot accumulates clock64() cycles per phase of the
+micro-step loop and stores them at the end of the launch.
+
+Workload = bench.py's headline: KukaButtonGymEnv-v0, 4096 envs, T = 128, bench seeds and inputs, 3 warm-up rollouts, then LAUNCHES measured
+rollouts.  Per phase it prints cycles per physics step (median and max over slots), the phase's share of the slowest slot of each launch
+(the slot that ends last bounds the launch), and the same for the whole slot.  The phase clocks add a few registers (more spills) and
+one clock read per mark, so the build runs a little slower than the shipped one: the split is the point, not the total."""
+import argparse, os, subprocess, sys
+import numpy as np
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "robotics-rl-srl_b200"))
+import torch
+from srl_sim._abi import load_cuda_library
+from srl_sim.backend import Backend
+from srl_sim.model import load_kuka_scene
+
+PHASES = ["kinematics + collision", "IK (float64 7x7)", "dynamics (CRBA + RNEA)", "Cholesky + M^-1", "v0 + row set-up + scaling + Euler",
+          "fast sweeps", "general loop", "env logic / loads / stores"]
+NPH = len(PHASES)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--launches", type=int, default=5)
+    ap.add_argument("--seed", type=int, default=0)
+    args = ap.parse_args()
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        print("device:", q.stdout.strip())
+    except Exception as ex:  # noqa: BLE001 -- the table is still valid without the card line
+        print("device: nvidia-smi unavailable (%r)" % (ex,))
+    n, T = 4096, 128
+    lib = load_cuda_library()
+    be = Backend(lib, 0)
+    st = be.stream()
+    # bench.py's workload_spec("kuka") / make_inputs / measure_b200 at rank 0
+    sim = be.make_sim("KukaButtonGymEnv-v0", n, seed=args.seed, model_blob=load_kuka_scene().blob,
+                      is_discrete=True, random_target=False, force_down=True, action_repeat=1, max_distance=0.8)
+    sim.reset(stream=st)
+    rng = np.random.default_rng(args.seed)
+    acts = be.from_host(rng.integers(0, 6, (T, n), dtype=np.int32))
+    noise = be.from_host(rng.normal(0, 0.01, (T, n)).astype(np.float32))
+    obs = be.zeros((T, n, 3), np.float32); rew = be.zeros((T, n), np.float32); done = be.zeros((T, n), np.uint8)
+    ep_ret = be.zeros((T, n), np.float32); ep_len = be.zeros((T, n), np.int32)
+    for _ in range(3):
+        sim.rollout(T, acts, noise, obs, rew, done, ep_ret, ep_len, stream=st)
+    torch.cuda.synchronize()
+    words = np.zeros((1 << 13, NPH + 1), np.uint64)
+    per_step = []          # [launch] -> (live slots, NPH) cycles per physics step
+    slowest = []           # [launch] -> (NPH,) cycles of the slowest slot
+    ms = []
+    for _ in range(args.launches):
+        words[:] = 0
+        sim.rollout(T, acts, noise, obs, rew, done, ep_ret, ep_len, stream=st)
+        torch.cuda.synchronize()
+        ms.append(sim.last_kernel_ms())
+        rc = sim._lib.srl_sim_get_state(sim.handle, 98, words.ctypes.data, words.nbytes)
+        assert rc == 0, "srl_sim_get_state(98) failed: not a -DKK_PHASES build?"
+        w = words.astype(np.float64)
+        live = w[:, NPH] > 0
+        cyc, nphys = w[live, :NPH], w[live, NPH]
+        per_step.append(cyc / nphys[:, None])
+        slowest.append(cyc[np.argmax(cyc.sum(axis=1))])
+    ps = np.concatenate(per_step)
+    sl = np.mean(slowest, axis=0)
+    print("KukaButtonGymEnv-v0, %d envs x T = %d, %d live slots, %d launches after 3 warm-ups: %s ms per launch (phase-clock build)"
+          % (n, T, per_step[0].shape[0], args.launches, " ".join("%.3f" % x for x in ms)))
+    print("%-36s %14s %14s %16s" % ("phase", "median cyc/step", "max cyc/step", "slowest slot %"))
+    for k in range(NPH):
+        print("%-36s %14.0f %14.0f %15.1f%%" % (PHASES[k], np.median(ps[:, k]), np.max(ps[:, k]), 100.0 * sl[k] / sl.sum()))
+    tot = ps.sum(axis=1)
+    print("%-36s %14.0f %14.0f %15.1f%%" % ("total", np.median(tot), np.max(tot), 100.0))
+    print("slowest slot: %.0f cycles per launch = %.3f ms at 1.98 GHz" % (sl.sum(), sl.sum() / 1.98e6))
+
+
+if __name__ == "__main__":
+    main()
