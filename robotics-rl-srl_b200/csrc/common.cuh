@@ -26,7 +26,8 @@ struct MobileDev {
     double2* ep;    // [N] {running episode return, running episode length}
 };
 
-struct KukaDev;  // kuka.cuh
+struct KukaDev;   // kuka_kernels.cu
+struct KukaNext;
 
 #define SRL_HOST_MAX_CHUNKS 16
 
@@ -43,7 +44,7 @@ struct srl_sim {
     MobileDev mob_alt;  // the other half of the double buffer (rollouts write here, then swap)
     int mobile_block;   // CTA-size override (0 = heuristic)
     KukaDev* kuka;
-    void* kuka_next;    // next-episode records (kuka_kernels.cu: KukaNextHost), only with srl_cfg.prefetch_resets
+    KukaNext* kuka_next; // next-episode records, only with srl_cfg.prefetch_resets (nullptr: off)
     cudaEvent_t pf_ev;  // end of the last bulk record fill (srl_sim_prefetch_resets); the next rollout launch waits for it
     bool pf_pending;
     cudaEvent_t roll_ev; // end of the last rollout launch of a handle with records; a bulk fill waits for it

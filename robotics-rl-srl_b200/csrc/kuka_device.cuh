@@ -1,4 +1,5 @@
-// Kuka button-push physics, device side (sm_90a), one thread per environment.
+// Kuka button-push physics, device side (sm_90a): one env's applyAction + stepSimulation, for both layouts of kuka_kernel (one thread
+// per env, or a group of four lanes per env whose once-per-step phases are in kuka_coop.cuh).
 //
 // One call of kuka_physics_step() == Kuka.applyAction's IK + 12 motor set-points
 // (environments/kuka_gym/kuka.py:142-187) followed by one p.stepSimulation()
@@ -22,27 +23,7 @@
 #include "kuka_coop.cuh"
 
 #define KK_DEV __device__ __forceinline__
-// Code-shape switches (see DESIGN.md "Kernel code shape"): per-body passes as rolled loops over
-// thread-local arrays (small code, LDL latency) or fully unrolled register code (large code, instruction-fetch bound).
-#ifndef KK_ROLL_IK
-#define KK_ROLL_IK 0
-#endif
-#ifndef KK_ROLL_DYN
-#define KK_ROLL_DYN 0
-#endif
-// Sweeps per loop iteration (2 lets ptxas rotate the lam registers instead of copying them, but doubles the loop body beyond the ~6 KB L0
-// instruction cache: measured slower).  The row updates are scalar FFMAs: sm_90 has no packed FP32 FMA (`fma.rn.f32x2`).
-#ifndef KK_SWEEP_UNROLL
-#define KK_SWEEP_UNROLL 1
-#endif
-// a second copy of the sweep loop without the contact watch, taken when no lane of the warp has a contact row to watch
-#ifndef KK_SWEEP_TIGHT
-#define KK_SWEEP_TIGHT 1
-#endif
-// sweeps per iteration of the tight loop
-#ifndef KK_TIGHT_UNROLL
-#define KK_TIGHT_UNROLL 1
-#endif
+// The sweep's row updates are scalar FFMAs: sm_90 has no packed FP32 FMA (`fma.rn.f32x2`).
 // Measured and dropped: folding the previous row's contribution into the impulse update ("deferred" form:
 // shorter loop-carried path, one more FFMA per row -- slower, the saturating form is already issue-bound), and the
 // unscaled sweep with FMNMX clamps (round 1's form).
@@ -147,10 +128,10 @@ KK_DEV void sphere_cylinder(f3 s, float r, float cx, float cy, float z0, float z
 // streamed from L2 every step -- 58% of all stall samples were `no_inst` (instruction fetch).  The per-body passes are
 // therefore ROLLED loops over the 12 bodies with their arrays in thread-local memory: a few hundred instructions that
 // stay resident in the instruction caches.
-template <bool WITH_CONTACTS, bool TWOB>
+template <bool TWOB>
 KK_DEV void kuka_fk(const KukaParams& P, KukaEnv& e, KukaKin& k, KukaContacts& ct) {
     float R[9], R7[9];
-    float Rall[WITH_CONTACTS ? KK_NB : 1][9];  // per-body rotations for the sphere loop (local memory)
+    float Rall[KK_NB][9];  // per-body rotations for the sphere loop (local memory)
     float ql[KK_NB];
 #pragma unroll
     for (int i = 0; i < KK_NB; ++i) ql[i] = e.q[i];
@@ -160,7 +141,7 @@ KK_DEV void kuka_fk(const KukaParams& P, KukaEnv& e, KukaKin& k, KukaContacts& c
     for (int t = 0; t < 9; ++t) R7[t] = R[t];
     int cbutton = 0, ctable = 0, cany0 = 0, cany1 = 0;
     float zmin_body = 1e30f;
-    if (WITH_CONTACTS) ct.n = 0;
+    ct.n = 0;
     const float bz = e.bbz;
     const float disc0 = bz + P.glider_z + e.qb + P.disc_z0, disc1 = bz + P.glider_z + e.qb + P.disc_z1;
     const float b2z = P.btn_base[2];
@@ -227,16 +208,14 @@ KK_DEV void kuka_fk(const KukaParams& P, KukaEnv& e, KukaKin& k, KukaContacts& c
             for (int t2 = 0; t2 < 9; ++t2) R7[t2] = R[t2];
             p7 = p;
         }
-        if (WITH_CONTACTS) {
 #pragma unroll
-            for (int t2 = 0; t2 < 9; ++t2) Rall[i][t2] = R[t2];
-            if (i >= P.sph_min_body) zmin_body = fminf(zmin_body, p.z);
-        }
+        for (int t2 = 0; t2 < 9; ++t2) Rall[i][t2] = R[t2];
+        if (i >= P.sph_min_body) zmin_body = fminf(zmin_body, p.z);
     }
     // Collision detection: ONE copy of the sphere-vs-shape code, runtime loop over the spheres.  The whole loop is skipped
     // while the lowest sphere-carrying body frame is more than (reach + margin) above every shape -- most of an episode
     // (this loop was a visible share of the kernel's stall samples before the test).
-    if (WITH_CONTACTS && zmin_body - P.sph_reach - zmax_shapes <= P.cdist) {
+    if (zmin_body - P.sph_reach - zmax_shapes <= P.cdist) {
 #pragma unroll 1
         for (int sidx = 0; sidx < P.nsph; ++sidx) {
             const int b = P.sph_body[sidx];
@@ -273,7 +252,8 @@ KK_DEV void kuka_fk(const KukaParams& P, KukaEnv& e, KukaKin& k, KukaContacts& c
             }
         }
     }
-    if (WITH_CONTACTS) { e.cbutton = cbutton; e.ctable = ctable; if (TWOB) { e.cany0 = cany0; e.cany1 = cany1; } }
+    e.cbutton = cbutton; e.ctable = ctable;
+    if (TWOB) { e.cany0 = cany0; e.cany1 = cany1; }
     e.grip[0] = k.c[8].x; e.grip[1] = k.c[8].y; e.grip[2] = k.c[8].z;   // getLinkState(kuka, 8)[0]: COM of link 8
     e.eepos[0] = k.p[6].x; e.eepos[1] = k.p[6].y; e.eepos[2] = k.p[6].z;
 }
@@ -296,91 +276,10 @@ KK_DEV void quat_from_matrix(const float* R, float* q) {
     }
 }
 
-#if KK_ROLL_IK
 // One damped-least-squares IK iteration at the current joint state (pybullet 1.8.6 / BussIK DLS):
 // dtheta = (J^T J + lambda I)^-1 J^T e over the 7 arm joints.  The 7x7 normal equations are formed and
 // solved in float64: they square the Jacobian's condition number, which float32 cannot afford.
-// Rolled loops over thread-local arrays (see the code-size note above kuka_fk).
-KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float* q_ik) {
-    constexpr int n = 7;
-    float J[n][6];
-    const f3 pe = k.p[6];
-#pragma unroll 1
-    for (int j = 0; j < n; ++j) {
-        const f3 aj = k.a[j];
-        const f3 l = cross3(aj, pe - k.p[j]);
-        J[j][0] = l.x; J[j][1] = l.y; J[j][2] = l.z; J[j][3] = aj.x; J[j][4] = aj.y; J[j][5] = aj.z;
-    }
-    float err[6];
-    err[0] = e.ee[0] - pe.x; err[1] = e.ee[1] - pe.y; err[2] = e.ee[2] - pe.z;
-    float qc[4];
-    quat_from_matrix(k.R6, qc);
-    const float cx = -qc[0], cy = -qc[1], cz = -qc[2], cw = qc[3];
-    const float dx = P.ikq[3] * cx + P.ikq[0] * cw + P.ikq[1] * cz - P.ikq[2] * cy;
-    const float dy = P.ikq[3] * cy - P.ikq[0] * cz + P.ikq[1] * cw + P.ikq[2] * cx;
-    const float dz = P.ikq[3] * cz + P.ikq[0] * cy - P.ikq[1] * cx + P.ikq[2] * cw;
-    const float dw = P.ikq[3] * cw - P.ikq[0] * cx - P.ikq[1] * cy - P.ikq[2] * cz;
-    const float vn = sqrtf(dx * dx + dy * dy + dz * dz);
-    // angle = 2 atan2(|v|, w) (== btQuaternion::getAngle, but well conditioned for small angles in fp32)
-    float angle = 2.0f * atan2f(vn, dw);
-    if (angle > 3.14159265358979f) angle -= 6.28318530717959f;
-    if (vn > 1e-12f) { const float sc = angle / vn; err[3] = sc * dx; err[4] = sc * dy; err[5] = sc * dz; }
-    else { err[3] = err[4] = err[5] = 0.f; }
-    double A[n][n], b[n];
-#pragma unroll 1
-    for (int i = 0; i < n; ++i) {
-#pragma unroll 1
-        for (int j = 0; j <= i; ++j) {
-            double acc = 0.0;
-#pragma unroll
-            for (int r = 0; r < 6; ++r) acc = fma((double)J[i][r], (double)J[j][r], acc);
-            A[i][j] = acc;
-        }
-        A[i][i] += P.ik_damp;
-        double acc = 0.0;
-#pragma unroll
-        for (int r = 0; r < 6; ++r) acc = fma((double)J[i][r], (double)err[r], acc);
-        b[i] = acc;
-    }
-    // Cholesky A = L L^T (A is SPD thanks to the damping), forward/back substitution
-#pragma unroll 1
-    for (int j = 0; j < n; ++j) {
-        double d = A[j][j];
-        for (int kk = 0; kk < j; ++kk) d -= A[j][kk] * A[j][kk];
-        const double inv = rsqrt(d);
-        A[j][j] = inv;  // store 1 / L_jj
-#pragma unroll 1
-        for (int i = j + 1; i < n; ++i) {
-            double acc = A[i][j];
-            for (int kk = 0; kk < j; ++kk) acc -= A[i][kk] * A[j][kk];
-            A[i][j] = acc * inv;
-        }
-    }
-#pragma unroll 1
-    for (int i = 0; i < n; ++i) {
-        double acc = b[i];
-        for (int kk = 0; kk < i; ++kk) acc -= A[i][kk] * b[kk];
-        b[i] = acc * A[i][i];
-    }
-#pragma unroll 1
-    for (int i = n - 1; i >= 0; --i) {
-        double acc = b[i];
-        for (int kk = i + 1; kk < n; ++kk) acc -= A[kk][i] * b[kk];
-        b[i] = acc * A[i][i];
-    }
-    double mx = 0.0;
-#pragma unroll
-    for (int i = 0; i < n; ++i) mx = fmax(mx, fabs(b[i]));
-    const double max_angle = 0.78539816339744830962;  // BussIK MaxAngleDLS = 45 degrees
-    const double scale = mx > max_angle ? max_angle / mx : 1.0;
-#pragma unroll
-    for (int i = 0; i < n; ++i) q_ik[i] = e.q[i] + (float)(scale * b[i]);
-}
-
-#else
-// One damped-least-squares IK iteration at the current joint state (pybullet 1.8.6 / BussIK DLS):
-// dtheta = (J^T J + lambda I)^-1 J^T e over the 7 arm joints.  The 7x7 normal equations are formed and
-// solved in float64: they square the Jacobian's condition number, which float32 cannot afford.
+// Fully unrolled: rolled loops over thread-local arrays (smaller code) were local-memory-latency bound, measured slower.
 KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float* q_ik) {
     constexpr int n = 7;
     float J[6][n];
@@ -459,88 +358,9 @@ KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, flo
     for (int i = 0; i < n; ++i) q_ik[i] = e.q[i] + (float)(scale * b[i]);
 }
 
-#endif
-#if KK_ROLL_DYN
-// Mass matrix (lower triangle, M[i][j], j <= i) by the composite-rigid-body algorithm and bias torques
-// (gravity, velocity products, Bullet link damping) by recursive Newton-Euler, both in world coordinates
-// about the world origin: sub-tree quantities accumulate by plain addition.  Rolled per-body loops.
-KK_DEV void kuka_dynamics(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float (&M)[KK_NB][KK_NB], float* bias) {
-    float qdl[KK_NB];
-#pragma unroll
-    for (int i = 0; i < KK_NB; ++i) qdl[i] = e.qd[i];
-    f3 nn[KK_NB], ff[KK_NB];          // body wrenches about the origin, then sub-tree sums
-    float cm[KK_NB]; f3 ch[KK_NB]; float cI[KK_NB][6];  // composite mass, first moment, inertia about the origin
-    // ---- RNEA forward pass + body wrenches (running parent state; the second finger restarts from body 7) ----
-    f3 w = mk3(0.f, 0.f, 0.f), vO = w, aw = w, av = mk3(0.f, 0.f, -P.gz);  // gravity as a fictitious base acceleration
-    f3 w7 = w, vO7 = w, aw7 = w, av7 = av;
-#pragma unroll 1
-    for (int i = 0; i < KK_NB; ++i) {
-        if (i == 10) { w = w7; vO = vO7; aw = aw7; av = av7; }
-        const float qd = qdl[i];
-        const f3 ai = k.a[i], pvi = k.pv[i];
-        const f3 awn = aw + qd * cross3(w, ai);
-        const f3 avn = av + qd * (cross3(w, pvi) + cross3(vO, ai));
-        w = w + qd * ai;
-        vO = vO + qd * pvi;
-        aw = awn; av = avn;
-        if (i == 7) { w7 = w; vO7 = vO; aw7 = aw; av7 = av; }
-        // spatial inertia about the origin: m, h = m c, I_O = Iw + m (|c|^2 1 - c c^T)
-        const float m = P.mass[i];
-        const f3 c = k.c[i];
-        const f3 h = m * c;
-        float Iw[6], IO[6];
-#pragma unroll
-        for (int t = 0; t < 6; ++t) Iw[t] = k.Iw[i][t];
-        IO[0] = Iw[0] + m * (c.y * c.y + c.z * c.z);
-        IO[1] = Iw[1] - m * c.x * c.y;
-        IO[2] = Iw[2] - m * c.x * c.z;
-        IO[3] = Iw[3] + m * (c.x * c.x + c.z * c.z);
-        IO[4] = Iw[4] - m * c.y * c.z;
-        IO[5] = Iw[5] + m * (c.x * c.x + c.y * c.y);
-        cm[i] = m; ch[i] = h;
-#pragma unroll
-        for (int t = 0; t < 6; ++t) cI[i][t] = IO[t];
-        const f3 Lv = symv(IO, w) + cross3(h, vO);
-        const f3 Pv = m * vO + cross3(w, h);
-        const f3 La = symv(IO, aw) + cross3(h, av);
-        const f3 Pa = m * av + cross3(aw, h);
-        f3 n = La + cross3(w, Lv) + cross3(vO, Pv);
-        f3 f = Pa + cross3(w, Pv);
-        // btMultiBody link damping (linear/angular 0.04, K1 = K2): resisting wrench added to the bias
-        const f3 vc = vO + cross3(w, c);
-        const f3 F = (P.kl * m * (1.0f + norm3(vc))) * vc;
-        const f3 T = (P.ka * (1.0f + norm3(w))) * symv(Iw, w);
-        nn[i] = n + T + cross3(c, F);
-        ff[i] = f + F;
-    }
-    // ---- backward pass: bias_i = s_i . (wrench of the sub-tree); CRBA: M_ij = s_i . (I^c_j s_j), i ancestor-or-self of j ----
-#pragma unroll 1
-    for (int j = KK_NB - 1; j >= 0; --j) {
-        const f3 aj = k.a[j], pvj = k.pv[j];
-        const f3 nj = nn[j], fj = ff[j];
-        bias[j] = dot3(aj, nj) + dot3(pvj, fj);
-        const float mj = cm[j]; const f3 hj = ch[j];
-        float Ij[6];
-#pragma unroll
-        for (int t = 0; t < 6; ++t) Ij[t] = cI[j][t];
-        const f3 Pm = mj * pvj + cross3(aj, hj);              // linear momentum of the composite under unit joint rate
-        const f3 Lm = symv(Ij, aj) + cross3(hj, pvj);         // angular momentum about the origin
-        for (int i = 0; i <= j; ++i) M[j][i] = 0.f;
-        for (int i = j; i >= 0; i = KK_PAR(i)) M[j][i] = dot3(k.a[i], Lm) + dot3(k.pv[i], Pm);
-        const int pa = KK_PAR(j);
-        if (pa >= 0) {
-            nn[pa] = nn[pa] + nj; ff[pa] = ff[pa] + fj;
-            cm[pa] += mj; ch[pa] = ch[pa] + hj;
-#pragma unroll
-            for (int t = 0; t < 6; ++t) cI[pa][t] += Ij[t];
-        }
-    }
-}
-
-#else
 // Mass matrix (lower triangle, m[i][j], j <= i) by the composite-rigid-body algorithm and bias torques
 // (gravity, velocity products, Bullet link damping) by recursive Newton-Euler, both in world coordinates
-// about the world origin: sub-tree quantities accumulate by plain addition.
+// about the world origin: sub-tree quantities accumulate by plain addition.  Fully unrolled, like kuka_ik (rolled per-body loops: slower).
 KK_DEV void kuka_dynamics(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float (&M)[KK_NB][KK_NB], float* bias) {
     f3 pv[KK_NB];  // linear part of the joint motion vector about the origin: p x a
 #pragma unroll
@@ -628,7 +448,6 @@ KK_DEV void kuka_dynamics(const KukaParams& P, const KukaEnv& e, const KukaKin& 
     }
 }
 
-#endif
 // In-place: M (lower) -> A = M^-1 (lower triangle valid), via Cholesky and triangular inverse.
 KK_DEV void kuka_spd_inverse(float (&M)[KK_NB][KK_NB]) {
     constexpr int n = KK_NB;
@@ -677,7 +496,7 @@ KK_DEV void kuka_spd_inverse(float (&M)[KK_NB][KK_NB]) {
 #define KK_A(i, j) ((i) >= (j) ? A[i][j] : A[j][i])
 
 // One applyAction + stepSimulation.  `k`/`ct` hold the kinematics / contacts of the CURRENT configuration
-// (computed by the caller with kuka_fk<true>); on return q, qd, qb, qdb are advanced by one time step.
+// (computed by the caller with kuka_fk); on return q, qd, qb, qdb are advanced by one time step.
 // JOINTS: use_inverse_kinematics = False (action_joints): the 7 arm set-points are given (`q_joints`), no IK (kuka.py:158-161).
 // TWOB: Kuka2ButtonGymEnv -- a second button glider (DoF KK_NB + 1) with the same motor / limit rows, right after the first.
 // COOP: the env is a group of 4 lanes (kuka_coop.cuh): kinematics, contact manifold, mass-matrix inverse, bias and contact rows come from
@@ -724,23 +543,10 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         kuka_spd_inverse(A);
         KK_PH(ph, KK_PH_CHOL);
     } else {
-#if KK_ROLL_DYN
-    {
-        float Mloc[KK_NB][KK_NB], bloc[KK_NB];  // thread-local (dynamically indexed by the rolled loops)
-        kuka_dynamics(P, e, k, Mloc, bloc);
-#pragma unroll
-        for (int i = 0; i < KK_NB; ++i) {       // -> registers (static indices only from here on)
-            bias[i] = bloc[i];
-#pragma unroll
-            for (int j = 0; j <= i; ++j) A[i][j] = Mloc[i][j];
-        }
-    }
-#else
-    kuka_dynamics(P, e, k, A, bias);
-#endif
-    KK_PH(ph, KK_PH_DYN);
-    kuka_spd_inverse(A);
-    KK_PH(ph, KK_PH_CHOL);
+        kuka_dynamics(P, e, k, A, bias);
+        KK_PH(ph, KK_PH_DYN);
+        kuka_spd_inverse(A);
+        KK_PH(ph, KK_PH_CHOL);
     }
     float v[ND];
     {
@@ -961,24 +767,24 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         if (P.iters > 0) {
             int left = P.iters;
             asm volatile("mov.u32 %0, %0;" : "+r"(left));
-#if defined(__CUDA_ARCH__) && KK_SWEEP_TIGHT
+#if defined(__CUDA_ARCH__)
             // most warp-sweeps watch no contact in ANY lane: those run a loop that is nothing but the rows and one
             // back edge.  Warp-uniform choice: no divergence.
             const bool quiet = __all_sync(__activemask(), nc == 0);
 #else
             const bool quiet = false;
 #endif
+            // one sweep per loop iteration: two let ptxas rotate the lam registers instead of copying them, but double the loop body beyond
+            // the ~6 KB L0 instruction cache (measured slower)
             if (quiet) {
-                constexpr int tight_unroll = KK_TIGHT_UNROLL;
-#pragma unroll tight_unroll
+#pragma unroll 1
                 do { KK_SWEEP_BUTTONS() KK_MOTOR_ROWS() KK_PROBE_SWEEP() } while (--left > 0);
                 it = P.iters;
             } else if constexpr (!COOP) {
                 // one thread per env (32 envs per warp, batches >= 16 384): nearly every warp holds SOME env with a candidate contact, and every
                 // lane pays for what one lane does -- so the watched rows are re-tested with their 14-term dot after each sweep by the lanes that
                 // have any (the incremental form below made every lane carry four rows, which was much slower at 32 768 envs)
-                constexpr int sweep_unroll = KK_SWEEP_UNROLL;
-#pragma unroll sweep_unroll
+#pragma unroll 1
                 do {
                     KK_SWEEP_BUTTONS()
                     KK_MOTOR_ROWS()
@@ -1023,8 +829,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
                     __syncwarp(gmask);
 #endif
                 }
-                constexpr int sweep_unroll = KK_SWEEP_UNROLL;
-#pragma unroll sweep_unroll
+#pragma unroll 1
                 do {
                     KK_SWEEP_BUTTONS()
                     KK_MOTOR_ROWS_WATCH()

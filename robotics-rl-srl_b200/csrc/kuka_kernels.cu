@@ -4,13 +4,13 @@
 // (environments/kuka_gym/kuka_button_gym_env.py:214-281,293-368,422-463), Kuka.applyAction
 // (environments/kuka_gym/kuka.py:118-187) and the PyBullet calls behind them.
 //
-// Mapping: ONE THREAD PER ENV, all dynamic state in registers for the whole fused rollout.  The projected
-// Gauss-Seidel solve (150 sweeps x >= 13 strictly sequential rows) is a dependency chain that no amount of
-// intra-env parallelism shortens, so lanes are not spent on it; instead `envs_per_warp` < 32 spreads a small
-// batch over all 592 warp schedulers (4096 envs -> ~600 warps of 7 live lanes), which also bounds the cost of
-// the divergent 5-step reset to the few envs sharing a warp.  The robot model arrives as a __grid_constant__
-// parameter block (constant bank, folded into FFMA operands).  HBM traffic is the SoA state once per launch
-// (float4 / int4 records, coalesced) plus action + noise in and obs + reward + done out per step.
+// Mapping: all dynamic state of an env in registers for the whole fused rollout.  By default an env is a GROUP of 4 lanes
+// (kuka_coop.cuh), which share out the once-per-step kinematics and dynamics and run the projected Gauss-Seidel solve (150 sweeps x
+// >= 13 strictly sequential rows, a chain no intra-env parallelism shortens) redundantly; `envs_per_warp` <= 8 spreads the batch at one
+// warp per warp scheduler.  One thread per env is the layout for batches that need more than 8 envs per warp (above 4 224 envs on
+// an H100).  With next-episode records on (KukaNext), 4096 envs run at 7 envs per warp instead of 8, so that every warp keeps the idle
+// slot that produces them.  The robot model arrives as a __grid_constant__ parameter block (constant bank, folded into FFMA operands).  HBM traffic
+// is the SoA state once per launch (float4 / int4 records, coalesced) plus action + noise in and obs + reward + done out per step.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -19,7 +19,8 @@
 #include "kuka_device.cuh"
 #include "render_core.h"
 
-struct KukaDev {
+// Per-env state in HBM, one 16-byte record per array: the live state (KukaDev) and the next-episode records (KukaNext) alike.
+struct KukaState {
     float4* q[3];    // [N] joint positions  (12 floats as 3 x float4)
     float4* qd[3];   // [N] joint velocities
     float4* misc0;   // ee.x ee.y ee.z qb
@@ -30,6 +31,9 @@ struct KukaDev {
     int4*   cnt;     // counter, n_contacts, n_outside, terminated | cbutton << 1 | ctable << 2
     int4*   cnt2;    // episode, total_steps, ep_len, moving button: high word of the float64 target y / two buttons: n_contacts[1]
     float4* btn2;    // two buttons only: second glider q, qd, second button base x, y
+};
+
+struct KukaDev : KukaState {
     KukaParams P;
     int epw;         // live env slots per warp (lanes, or groups of 4 lanes when coop)
     int coop;        // 1: four lanes per env (kuka_coop.cuh), epw <= 8
@@ -47,16 +51,11 @@ struct KukaDev {
 // clean, but its long launches shared schedulers with 2-4 following step launches and doubled their duration.  A helper CTA on the
 // last SM worked too, but cannot serve enough records once an env takes 4 lanes.)
 // op = PREFETCH as a launch of its own (srl_sim_prefetch_resets) remains as the bulk fill after an explicit reset of all envs.
-// Same member names as KukaDev's state arrays: env_load / env_store work on either.
-struct KukaNext {
-    float4* q[3]; float4* qd[3];
-    float4 *misc0, *misc1, *tgt, *grip, *eepos;
-    int4 *cnt, *cnt2;
-    float4* btn2;
+struct KukaNext : KukaState {
     uint8_t* valid;     // [N] 1 = record complete and not yet consumed
     int32_t* episode;   // [N] episode index the record was produced for (a record for another episode is dropped)
     uint8_t* progress;  // [N] random micro-steps of reset() already applied to an incomplete record (0 = not started)
-    int helper;         // 1: the LAST CTA of a rollout launch is the helper CTA that advances incomplete records (see kuka_kernel)
+    int helper;         // 1 (rollout launches): the first idle slot of every warp advances an incomplete record of its warp's envs (see kuka_kernel)
 };
 
 namespace {
@@ -69,8 +68,8 @@ constexpr int N_CONTACTS_BEFORE_TERMINATION = 5, N_STEPS_OUTSIDE_SAFETY_SPHERE =
 template <bool CG, class T>
 KK_DEV T ld_state(const T* p) { return CG ? __ldcg(p) : *p; }
 
-template <bool TWOB, bool CG = false, class Arr = KukaDev>
-KK_DEV void env_load(const Arr& d, int i, KukaEnv& e) {
+template <bool TWOB, bool CG = false>
+KK_DEV void env_load(const KukaState& d, int i, KukaEnv& e) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         const float4 a = ld_state<CG>(d.q[k] + i), b = ld_state<CG>(d.qd[k] + i);
@@ -98,8 +97,8 @@ KK_DEV void env_load(const Arr& d, int i, KukaEnv& e) {
     }
 }
 
-template <bool TWOB, class Arr = KukaDev>
-KK_DEV void env_store(const Arr& d, int i, const KukaEnv& e) {
+template <bool TWOB>
+KK_DEV void env_store(const KukaState& d, int i, const KukaEnv& e) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         d.q[k][i] = make_float4(e.q[4 * k], e.q[4 * k + 1], e.q[4 * k + 2], e.q[4 * k + 3]);
@@ -395,7 +394,7 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
             if (TWOB) { e.cany0 = (fl >> 2) & 1; e.cany1 = (fl >> 3) & 1; }
             nc_reg = near ? (int)sc[KC_OFF_LINK + 7] : 0;
             KK_PH(ph, KK_PH_KIN);
-        } else { KK_PH(ph, KK_PH_ENV); kuka_fk<true, TWOB>(P, e, k, ct); KK_PH(ph, KK_PH_KIN); }
+        } else { KK_PH(ph, KK_PH_ENV); kuka_fk<TWOB>(P, e, k, ct); KK_PH(ph, KK_PH_KIN); }
         const int new_cb = e.cbutton, new_ct = e.ctable, new_a0 = TWOB ? e.cany0 : 0, new_a1 = TWOB ? e.cany1 : 0;
         if (pending) {
             // ---- _reward() (:428-463): manifold of the step that just ran, link states after it ----
@@ -659,85 +658,22 @@ __global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, floa
 }
 
 // ---- host side -------------------------------------------------------------------------------
+// the model part comes from kuka_params_from_blob (kuka_params.cuh); what depends on the env kind and srl_cfg is set here
 bool fill_params(const void* blob, size_t bytes, const srl_sim* s, KukaParams& P) {
     const double* d = (const double*)blob;
-    if (!blob || bytes < KM_HEADER_SIZE * sizeof(double) || d[KM_H_MAGIC] != KM_MAGIC || d[KM_H_VERSION] != KM_VERSION) {
-        srl_set_error("kuka: bad model blob (magic/version)"); return false;
-    }
-    if ((size_t)d[KM_H_TOTAL] * sizeof(double) != bytes || (int)d[KM_H_NBODY] != KK_NB || (int)d[KM_H_NSPHERE] > KM_MAX_SPHERES) {
-        srl_set_error("kuka: bad model blob (size / body count / sphere count)"); return false;
-    }
-    memset(&P, 0, sizeof(P));
+    if (const char* err = kuka_params_from_blob(d, bytes, s->cfg.timestep, P)) { srl_set_error("%s", err); return false; }
     const double* sc = d + (int)d[KM_H_SCENE_OFF];
-    const double dt = s->cfg.timestep > 0.f ? (double)s->cfg.timestep : sc[KM_SC_TIMESTEP];
-    static const int parent[KK_NB] = {-1, 0, 1, 2, 3, 4, 5, 6, 7, 8, 7, 10};
-    for (int i = 0; i < KK_NB; ++i) {
-        const double* r = d + (int)d[KM_H_BODY_OFF] + i * KM_BODY_STRIDE;
-        const double* c = d + (int)d[KM_H_CTRL_OFF] + i * KM_CTRL_STRIDE;
-        if ((int)r[KM_B_PARENT] != parent[i] || (int)r[KM_B_JTYPE] != 0) {
-            srl_set_error("kuka: the kernels are specialised for the 8-chain + two 2-link fingers revolute topology"); return false;
-        }
-        for (int a = 0; a < 3; ++a) { P.org[i][a] = (float)r[KM_B_ORIGIN + a]; P.axis[i][a] = (float)r[KM_B_AXIS + a]; P.com[i][a] = (float)r[KM_B_COM + a]; }
-        for (int a = 0; a < 9; ++a) P.rot[i][a] = (float)r[KM_B_ROT + a];
-        for (int a = 0; a < 6; ++a) P.Ic[i][a] = (float)r[KM_B_INERTIA + a];
-        P.mass[i] = (float)r[KM_B_MASS]; P.damping[i] = (float)r[KM_B_DAMPING];
-        P.lower[i] = (float)r[KM_B_LOWER]; P.upper[i] = (float)r[KM_B_UPPER];
-        P.kp_dt[i] = (float)(c[KM_C_KP] / dt); P.kd[i] = (float)c[KM_C_KD];
-        P.maxvel[i] = (float)c[KM_C_MAXVEL]; P.maximp[i] = (float)(c[KM_C_MAXFORCE] * dt);
-        P.tmode[i] = (int)c[KM_C_TARGET];
-        P.snap_q[i] = (float)r[KM_B_QINIT];
-    }
-    for (int i = 0; i < KK_NB; ++i) {
-        if (!(P.maximp[i] > 0.f)) { srl_set_error("kuka: every motor needs a positive force bound (the sweep carries impulses scaled to it)"); return false; }
-        const double sg = 2.0 * (double)P.maximp[i];
-        P.sat_sig[i] = (float)sg; P.sat_isig[i] = (float)(1.0 / sg); P.sat_isig2[i] = (float)(1.0 / (sg * sg));
-        for (int j = 0; j <= i; ++j) {
-            const double ss = sg * 2.0 * (double)P.maximp[j];
-            P.sat_ss[i * (i + 1) / 2 + j] = (float)ss; P.sat_iss[i * (i + 1) / 2 + j] = (float)(1.0 / ss);
-        }
-    }
-    P.nsph = (int)d[KM_H_NSPHERE];
-    P.sph_min_body = KK_NB; P.sph_reach = 0.f;
-    for (int k = 0; k < P.nsph; ++k) {
-        const double* sp = d + (int)d[KM_H_SPHERE_OFF] + k * KM_SPHERE_STRIDE;
-        P.sph_body[k] = (int)sp[KM_S_BODY]; P.sph_r[k] = (float)sp[KM_S_RADIUS];
-        for (int a = 0; a < 3; ++a) P.sph_c[k][a] = (float)sp[KM_S_CENTER + a];
-        if (P.sph_body[k] < P.sph_min_body) P.sph_min_body = P.sph_body[k];
-        const float reach = sqrtf(P.sph_c[k][0] * P.sph_c[k][0] + P.sph_c[k][1] * P.sph_c[k][1] + P.sph_c[k][2] * P.sph_c[k][2]) + P.sph_r[k];
-        if (reach > P.sph_reach) P.sph_reach = reach * 1.0001f;
-    }
-    for (int a = 0; a < 3; ++a) { P.base[a] = (float)sc[KM_SC_BASE_POS + a]; P.btn_base[a] = (float)sc[KM_SC_BUTTON_BASE + a]; P.ee_init[a] = (float)sc[KM_SC_EE_INIT + a]; }
-    P.gz = (float)sc[KM_SC_GRAVITY_Z]; P.dt = (float)dt; P.inv_dt = (float)(1.0 / dt);
     P.iters = s->cfg.solver_iterations > 0 ? s->cfg.solver_iterations : (int)sc[KM_SC_SOLVER_ITERS];
-    P.table_z = (float)sc[KM_SC_TABLE_TOP_Z]; P.txmin = (float)sc[KM_SC_TABLE_XMIN]; P.txmax = (float)sc[KM_SC_TABLE_XMAX];
-    P.tymin = (float)sc[KM_SC_TABLE_YMIN]; P.tymax = (float)sc[KM_SC_TABLE_YMAX];
-    P.glider_z = (float)sc[KM_SC_GLIDER_Z]; P.gl_lo = (float)sc[KM_SC_GLIDER_LOWER]; P.gl_hi = (float)sc[KM_SC_GLIDER_UPPER];
-    P.btn_minv = (float)(1.0 / sc[KM_SC_BUTTON_MASS]);
-    P.disc_r = (float)sc[KM_SC_DISC_RADIUS]; P.disc_z0 = (float)sc[KM_SC_DISC_Z0]; P.disc_z1 = (float)sc[KM_SC_DISC_Z1];
-    P.stack_r = (float)sc[KM_SC_STACK_RADIUS]; P.stack_top = (float)sc[KM_SC_STACK_TOP];
-    P.cdist = (float)sc[KM_SC_CONTACT_DIST]; P.mu = (float)sc[KM_SC_FRICTION]; P.erp = (float)sc[KM_SC_ERP];
-    P.kl = (float)sc[KM_SC_LIN_DAMPING]; P.ka = (float)sc[KM_SC_ANG_DAMPING];
     const bool two = s->kind == SRL_ENV_KUKA_2BUTTON;
     // small_constraints = not random_target (:239); Kuka2Button always uses the large box (kuka_2button_gym_env.py:78)
     const double* box = sc + ((s->cfg.random_target || two) ? KM_SC_BOX_LARGE : KM_SC_BOX_SMALL);
     for (int a = 0; a < 6; ++a) P.box[a] = (float)box[a];
-    for (int a = 0; a < 4; ++a) P.ikq[a] = (float)sc[KM_SC_IK_QUAT + a];
-    P.ik_damp = sc[KM_SC_IK_DAMPING];
-    P.ee_body = (int)sc[KM_SC_EE_BODY]; P.grip_body = (int)sc[KM_SC_GRIPPER_BODY];
-    if (P.ee_body != 6 || P.grip_body != 8) { srl_set_error("kuka: kernels assume IK link 6 and gripper link 8 (kuka.py:31-32)"); return false; }
-    P.target_h = (float)sc[KM_SC_TARGET_HEIGHT]; P.rand_x = (float)sc[KM_SC_RAND_X]; P.rand_y = (float)sc[KM_SC_RAND_Y];
-    P.btn_idle_imp = (float)sc[KM_SC_BTN_IDLE_IMPULSE]; P.btn_kp_dt = (float)(sc[KM_SC_BTN_KP] / dt); P.btn_kd = (float)sc[KM_SC_BTN_KD];
-    P.btn_target = (float)sc[KM_SC_BTN_TARGET]; P.btn_maximp = (float)(sc[KM_SC_BTN_MAXFORCE] * dt);
-    P.lim_maximp = (float)sc[KM_SC_LIMIT_MAX_IMPULSE]; P.lim_eps = (float)sc[KM_SC_LIMIT_EPS];
-    P.max_contacts = (int)sc[KM_SC_MAX_CONTACTS];
-    if (P.max_contacts > KK_MAXC) P.max_contacts = KK_MAXC;
     P.is_discrete = s->cfg.is_discrete; P.random_target = s->cfg.random_target; P.force_down = s->cfg.force_down;
     P.shape_reward = s->cfg.shape_reward; P.action_repeat = s->cfg.action_repeat; P.max_steps = s->max_steps;
     P.auto_reset = s->auto_reset; P.max_distance = s->cfg.max_distance;
     P.moving_button = s->kind == SRL_ENV_KUKA_MOVING_BUTTON;
     P.action_joints = s->cfg.action_joints != 0;
     P.two_buttons = two;
-    P.two_tgt_z = (float)(-0.2 + sc[KM_SC_TARGET_HEIGHT]);   // Z_TABLE + BUTTON_DISTANCE_HEIGHT (kuka_button_gym_env.py:26,35)
     if (two) {
         P.btn_base[1] = 0.125f;                               // kuka_2button_gym_env.py:49-57 (button 2 mirrors it at -0.125)
         // `use_null_space = True` (:80) -> calculateInverseKinematics(uid, link, pos, orn, ll, ul, jr, rp) (kuka.py:147-149).  RECALLED
@@ -745,17 +681,28 @@ bool fill_params(const void* blob, size_t bytes, const srl_sim* s, KukaParams& P
         // and without a jointDamping argument the server's default damping 0.5 per DoF applies (DESIGN.md section 4)
         P.ik_damp = 0.5;
     }
-    for (int j = 0; j < 7; ++j) P.qinit[j] = P.snap_q[j];   // snap_q still holds the initial joint vector here
     P.seed = s->seed; P.env_offset = s->cfg.global_env_offset;
     return true;
 }
 
-// one instantiation per (action_joints, two_buttons, four-lanes-per-env): the default kernel pays nothing for the variants
+int alloc_state(KukaState& a, size_t N) {
+    float4** f4[] = {&a.q[0], &a.q[1], &a.q[2], &a.qd[0], &a.qd[1], &a.qd[2], &a.misc0, &a.misc1, &a.tgt, &a.grip, &a.eepos, &a.btn2};
+    for (float4** p : f4) { SRL_CUDA_OK(cudaMalloc(p, N * sizeof(float4))); SRL_CUDA_OK(cudaMemset(*p, 0, N * sizeof(float4))); }
+    int4** i4[] = {&a.cnt, &a.cnt2};
+    for (int4** p : i4) { SRL_CUDA_OK(cudaMalloc(p, N * sizeof(int4))); SRL_CUDA_OK(cudaMemset(*p, 0, N * sizeof(int4))); }
+    return 0;
+}
+
+void free_state(KukaState& a) {
+    for (int k = 0; k < 3; ++k) { cudaFree(a.q[k]); cudaFree(a.qd[k]); }
+    cudaFree(a.misc0); cudaFree(a.misc1); cudaFree(a.tgt); cudaFree(a.grip); cudaFree(a.eepos); cudaFree(a.cnt); cudaFree(a.cnt2); cudaFree(a.btn2);
+}
+
 #define KUKA_SMEM_BYTES ((size_t)(((KC_CONST_WORDS + 31) / 32) * 32 + 32 * KC_ES) * sizeof(float))   /* 4 warps x 8 env slots */
 template <bool J, bool T2, bool PF, bool CO>
-cudaError_t kuka_launch_inst(const KukaDev* d, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions, const float* noise,
-                             const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret, int32_t* ep_len,
-                             float* snap, const KukaNext& nx) {
+cudaError_t kuka_launch_inst(const KukaDev& d, const KukaNext& nx, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions,
+                             const float* noise, const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret,
+                             int32_t* ep_len, float* snap) {
     const size_t smem = CO ? KUKA_SMEM_BYTES : 0;
     static bool attr_set = false;
     if (CO && !attr_set) {
@@ -763,32 +710,24 @@ cudaError_t kuka_launch_inst(const KukaDev* d, int grid, int block, cudaStream_t
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
-    kuka_kernel<J, T2, PF, CO><<<grid, block, smem, st>>>(*d, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap, nx);
+    kuka_kernel<J, T2, PF, CO><<<grid, block, smem, st>>>(d, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap, nx);
     return cudaGetLastError();
 }
-#define KUKA_LAUNCH(d, grid, block, st, ...)                                                                             \
-    do {                                                                                                                 \
-        const KukaNext nx0 = KukaNext{};                                                                                 \
-        cudaError_t le;                                                                                                  \
-        const int jt = ((d)->P.action_joints ? 1 : 0) | ((d)->P.two_buttons ? 2 : 0) | ((d)->coop ? 4 : 0);              \
-        switch (jt) {                                                                                                    \
-        case 0: le = kuka_launch_inst<false, false, false, false>(d, grid, block, st, __VA_ARGS__, nx0); break;          \
-        case 1: le = kuka_launch_inst<true, false, false, false>(d, grid, block, st, __VA_ARGS__, nx0); break;           \
-        case 2: le = kuka_launch_inst<false, true, false, false>(d, grid, block, st, __VA_ARGS__, nx0); break;           \
-        case 3: le = kuka_launch_inst<true, true, false, false>(d, grid, block, st, __VA_ARGS__, nx0); break;            \
-        case 4: le = kuka_launch_inst<false, false, false, true>(d, grid, block, st, __VA_ARGS__, nx0); break;           \
-        case 5: le = kuka_launch_inst<true, false, false, true>(d, grid, block, st, __VA_ARGS__, nx0); break;            \
-        case 6: le = kuka_launch_inst<false, true, false, true>(d, grid, block, st, __VA_ARGS__, nx0); break;            \
-        default: le = kuka_launch_inst<true, true, false, true>(d, grid, block, st, __VA_ARGS__, nx0); break;            \
-        }                                                                                                                \
-        SRL_CUDA_OK(le);                                                                                                 \
-    } while (0)
 
-// Host-side owner of the next-episode records of one handle (srl_sim::kuka_next); the kernel gets the pointer block by value.
-struct KukaNextHost {
-    KukaNext nx;
-    bool enabled;
-};
+// One instantiation per (action_joints, two_buttons, four lanes per env): the default kernel pays nothing for the variants.  With
+// next-episode records (`nx`, single-button kinds with IK actions only) the PREFETCH instantiation of the same layout.
+cudaError_t kuka_launch(const KukaDev& d, const KukaNext* nx, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions,
+                        const float* noise, const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret,
+                        int32_t* ep_len, float* snap) {
+    using Launch = decltype(&kuka_launch_inst<false, false, false, false>);
+    static const Launch plain[8] = {kuka_launch_inst<false, false, false, false>, kuka_launch_inst<true, false, false, false>,
+                                    kuka_launch_inst<false, true, false, false>,  kuka_launch_inst<true, true, false, false>,
+                                    kuka_launch_inst<false, false, false, true>,  kuka_launch_inst<true, false, false, true>,
+                                    kuka_launch_inst<false, true, false, true>,   kuka_launch_inst<true, true, false, true>};
+    const Launch launch = nx ? (d.coop ? kuka_launch_inst<false, false, true, true> : kuka_launch_inst<false, false, true, false>)
+                             : plain[(d.P.action_joints ? 1 : 0) | (d.P.two_buttons ? 2 : 0) | (d.coop ? 4 : 0)];
+    return launch(d, nx ? *nx : KukaNext{}, grid, block, st, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap);
+}
 
 void grid_for(const srl_sim* s, const KukaDev* d, int& grid, int& block) {
     const int warps = (s->n + d->epw - 1) / d->epw;
@@ -804,11 +743,7 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
     s->kuka = d;
     if (!fill_params(blob, bytes, s, d->P)) return 1;
     const size_t N = (size_t)s->n;
-    float4** f4[] = {&d->q[0], &d->q[1], &d->q[2], &d->qd[0], &d->qd[1], &d->qd[2], &d->misc0, &d->misc1, &d->tgt, &d->grip, &d->eepos};
-    for (float4** p : f4) { SRL_CUDA_OK(cudaMalloc(p, N * sizeof(float4))); SRL_CUDA_OK(cudaMemset(*p, 0, N * sizeof(float4))); }
-    SRL_CUDA_OK(cudaMalloc(&d->cnt, N * sizeof(int4))); SRL_CUDA_OK(cudaMemset(d->cnt, 0, N * sizeof(int4)));
-    SRL_CUDA_OK(cudaMalloc(&d->cnt2, N * sizeof(int4))); SRL_CUDA_OK(cudaMemset(d->cnt2, 0, N * sizeof(int4)));
-    SRL_CUDA_OK(cudaMalloc(&d->btn2, N * sizeof(float4))); SRL_CUDA_OK(cudaMemset(d->btn2, 0, N * sizeof(float4)));
+    if (alloc_state(*d, N)) return 1;
     // live lanes per warp: spread a small batch over every warp scheduler (4 per SM), ONE warp each -- the PGS
     // sweep of a single warp already fills its scheduler's issue slots, a second resident warp only adds latency
     const int sms = s->sms;
@@ -829,7 +764,7 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
     float* snap = nullptr;
     SRL_CUDA_OK(cudaMalloc(&snap, 32 * sizeof(float)));
     { const int save_epw = d->epw; d->epw = 1;
-      KUKA_LAUNCH(d, 1, 32, 0, 1, KUKA_OP_SETTLE, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, snap);
+      SRL_CUDA_OK(kuka_launch(*d, nullptr, 1, 32, 0, 1, KUKA_OP_SETTLE, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, snap));
       d->epw = save_epw; }
     SRL_CUDA_OK(cudaGetLastError());
     float h[32];
@@ -840,20 +775,15 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
     s->launches += 1;
     // opt-in next-episode records (single-button kinds with IK actions and auto-reset: the instantiation that exists)
     if (records) {
-        KukaNextHost* nh = new KukaNextHost();
-        memset(nh, 0, sizeof(*nh));
-        s->kuka_next = nh;
-        KukaNext& nx = nh->nx;
-        float4** g4[] = {&nx.q[0], &nx.q[1], &nx.q[2], &nx.qd[0], &nx.qd[1], &nx.qd[2], &nx.misc0, &nx.misc1, &nx.tgt, &nx.grip, &nx.eepos, &nx.btn2};
-        for (float4** p : g4) { SRL_CUDA_OK(cudaMalloc(p, N * sizeof(float4))); SRL_CUDA_OK(cudaMemset(*p, 0, N * sizeof(float4))); }
-        SRL_CUDA_OK(cudaMalloc(&nx.cnt, N * sizeof(int4))); SRL_CUDA_OK(cudaMemset(nx.cnt, 0, N * sizeof(int4)));
-        SRL_CUDA_OK(cudaMalloc(&nx.cnt2, N * sizeof(int4))); SRL_CUDA_OK(cudaMemset(nx.cnt2, 0, N * sizeof(int4)));
-        SRL_CUDA_OK(cudaMalloc(&nx.valid, N)); SRL_CUDA_OK(cudaMemset(nx.valid, 0, N));
-        SRL_CUDA_OK(cudaMalloc(&nx.episode, N * sizeof(int32_t))); SRL_CUDA_OK(cudaMemset(nx.episode, 0xff, N * sizeof(int32_t)));
-        SRL_CUDA_OK(cudaMalloc(&nx.progress, N)); SRL_CUDA_OK(cudaMemset(nx.progress, 0, N));
+        KukaNext* nx = new KukaNext();
+        memset(nx, 0, sizeof(*nx));
+        s->kuka_next = nx;
+        if (alloc_state(*nx, N)) return 1;
+        SRL_CUDA_OK(cudaMalloc(&nx->valid, N)); SRL_CUDA_OK(cudaMemset(nx->valid, 0, N));
+        SRL_CUDA_OK(cudaMalloc(&nx->episode, N * sizeof(int32_t))); SRL_CUDA_OK(cudaMemset(nx->episode, 0xff, N * sizeof(int32_t)));
+        SRL_CUDA_OK(cudaMalloc(&nx->progress, N)); SRL_CUDA_OK(cudaMemset(nx->progress, 0, N));
         SRL_CUDA_OK(cudaEventCreateWithFlags(&s->pf_ev, cudaEventDisableTiming));
         SRL_CUDA_OK(cudaEventCreateWithFlags(&s->roll_ev, cudaEventDisableTiming));
-        nh->enabled = true;
     }
     return 0;
 }
@@ -861,16 +791,13 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
 void kuka_free(srl_sim* s) {
     KukaDev* d = s->kuka;
     if (!d) return;
-    for (int k = 0; k < 3; ++k) { cudaFree(d->q[k]); cudaFree(d->qd[k]); }
-    cudaFree(d->misc0); cudaFree(d->misc1); cudaFree(d->tgt); cudaFree(d->grip); cudaFree(d->eepos); cudaFree(d->cnt); cudaFree(d->cnt2); cudaFree(d->btn2);
+    free_state(*d);
     delete d;
     s->kuka = nullptr;
-    if (KukaNextHost* nh = static_cast<KukaNextHost*>(s->kuka_next)) {
-        KukaNext& nx = nh->nx;
-        for (int k = 0; k < 3; ++k) { cudaFree(nx.q[k]); cudaFree(nx.qd[k]); }
-        cudaFree(nx.misc0); cudaFree(nx.misc1); cudaFree(nx.tgt); cudaFree(nx.grip); cudaFree(nx.eepos); cudaFree(nx.cnt); cudaFree(nx.cnt2);
-        cudaFree(nx.btn2); cudaFree(nx.valid); cudaFree(nx.episode); cudaFree(nx.progress);
-        delete nh;
+    if (KukaNext* nx = s->kuka_next) {
+        free_state(*nx);
+        cudaFree(nx->valid); cudaFree(nx->episode); cudaFree(nx->progress);
+        delete nx;
         s->kuka_next = nullptr;
         if (s->pf_ev) cudaEventDestroy(s->pf_ev);
         if (s->roll_ev) cudaEventDestroy(s->roll_ev);
@@ -880,7 +807,7 @@ void kuka_free(srl_sim* s) {
 int kuka_launch_reset(srl_sim* s, const uint8_t* mask, const double* draws, float* obs, cudaStream_t st) {
     KukaDev* d = s->kuka;
     int grid, block; grid_for(s, d, grid, block);
-    KUKA_LAUNCH(d, grid, block, st, s->n, KUKA_OP_RESET, 0, nullptr, nullptr, mask, draws, obs, nullptr, nullptr, nullptr, nullptr, nullptr);
+    SRL_CUDA_OK(kuka_launch(*d, nullptr, grid, block, st, s->n, KUKA_OP_RESET, 0, nullptr, nullptr, mask, draws, obs, nullptr, nullptr, nullptr, nullptr, nullptr));
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -889,20 +816,18 @@ int kuka_launch_rollout(srl_sim* s, int T, const void* actions, const float* noi
                         float* ep_ret, int32_t* ep_len, cudaStream_t st) {
     KukaDev* d = s->kuka;
     int grid, block; grid_for(s, d, grid, block);
-    const KukaNextHost* nh = static_cast<const KukaNextHost*>(s->kuka_next);
-    if (nh && nh->enabled) {    // the rollout path that takes a ready next-episode record instead of resetting inside the launch
+    if (s->kuka_next) {         // the rollout path that takes a ready next-episode record instead of resetting inside the launch
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         cudaStreamIsCapturing(st, &cap);
         const bool capturing = cap != cudaStreamCaptureStatusNone;   // events recorded outside a capture cannot be waited for inside it
         if (s->pf_pending && !capturing) { SRL_CUDA_OK(cudaStreamWaitEvent(st, s->pf_ev, 0)); s->pf_pending = false; }
-        KukaNext nx = nh->nx;
+        KukaNext nx = *s->kuka_next;
         nx.helper = 1;          // the first idle slot of every warp advances one incomplete record of its warp's envs by up to T micro-steps
-        if (d->coop) SRL_CUDA_OK((kuka_launch_inst<false, false, true, true>(d, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr, nx)));
-        else SRL_CUDA_OK((kuka_launch_inst<false, false, true, false>(d, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr, nx)));
+        SRL_CUDA_OK(kuka_launch(*d, &nx, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr));
         if (!capturing) { SRL_CUDA_OK(cudaEventRecord(s->roll_ev, st)); s->roll_ev_valid = true; }
     }
     else
-        KUKA_LAUNCH(d, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr);
+        SRL_CUDA_OK(kuka_launch(*d, nullptr, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr));
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -911,13 +836,11 @@ int kuka_launch_rollout(srl_sim* s, int T, const void* actions, const float* noi
 // run concurrently with step / rollout launches of the same handle (flag + fence hand-over, see KukaNext).  A no-op when the feature is off.
 int kuka_launch_prefetch(srl_sim* s, cudaStream_t st) {
     KukaDev* d = s->kuka;
-    const KukaNextHost* nh = static_cast<const KukaNextHost*>(s->kuka_next);
-    if (!nh || !nh->enabled) return 0;
+    if (!s->kuka_next) return 0;
     int grid, block; grid_for(s, d, grid, block);
-    // never concurrent with a rollout launch of the handle: its helper CTA writes the same records
+    // never concurrent with a rollout launch of the handle: its idle slots advance the same records
     if (s->roll_ev_valid) SRL_CUDA_OK(cudaStreamWaitEvent(st, s->roll_ev, 0));
-    if (d->coop) SRL_CUDA_OK((kuka_launch_inst<false, false, true, true>(d, grid, block, st, s->n, KUKA_OP_PREFETCH, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nh->nx)));
-    else SRL_CUDA_OK((kuka_launch_inst<false, false, true, false>(d, grid, block, st, s->n, KUKA_OP_PREFETCH, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nh->nx)));
+    SRL_CUDA_OK(kuka_launch(*d, s->kuka_next, grid, block, st, s->n, KUKA_OP_PREFETCH, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
     SRL_CUDA_OK(cudaEventRecord(s->pf_ev, st));
     s->pf_pending = true;
     s->launches += 1;
@@ -1021,13 +944,13 @@ int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
 #endif
     case SRL_F_NEXT_RECORD: {
         if (!need(3, 4)) return 1;
-        const KukaNextHost* nh = static_cast<const KukaNextHost*>(s->kuka_next);
+        const KukaNext* nx = s->kuka_next;
         for (size_t i = 0; i < N; ++i) { I[3 * i] = 0; I[3 * i + 1] = 0; I[3 * i + 2] = -1; }
-        if (nh && nh->enabled) {
+        if (nx) {
             std::vector<uint8_t> va(N), pr(N); std::vector<int32_t> ep(N);
-            SRL_CUDA_OK(cudaMemcpy(va.data(), nh->nx.valid, N, cudaMemcpyDeviceToHost));
-            SRL_CUDA_OK(cudaMemcpy(pr.data(), nh->nx.progress, N, cudaMemcpyDeviceToHost));
-            SRL_CUDA_OK(cudaMemcpy(ep.data(), nh->nx.episode, N * sizeof(int32_t), cudaMemcpyDeviceToHost));
+            SRL_CUDA_OK(cudaMemcpy(va.data(), nx->valid, N, cudaMemcpyDeviceToHost));
+            SRL_CUDA_OK(cudaMemcpy(pr.data(), nx->progress, N, cudaMemcpyDeviceToHost));
+            SRL_CUDA_OK(cudaMemcpy(ep.data(), nx->episode, N * sizeof(int32_t), cudaMemcpyDeviceToHost));
             for (size_t i = 0; i < N; ++i) { I[3 * i] = va[i]; I[3 * i + 1] = pr[i]; I[3 * i + 2] = ep[i]; }
         }
         return 0;

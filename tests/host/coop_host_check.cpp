@@ -1,5 +1,6 @@
 // Host check of csrc/kuka_coop.cuh (four lanes per env, phases through a scratch area) against the one-thread-per-env functions of
-// csrc/kuka_device.cuh, both compiled for the CPU: same model blob, random joint states, with and without contacts.
+// csrc/kuka_device.cuh, both compiled for the CPU: the model filled by the library's kuka_params_from_blob (csrc/kuka_params.cuh), random
+// joint states, with and without contacts.
 // Test infrastructure.  Build + run: tests/test_coop_host_cpu.py (g++ -O1 -ffp-contract=off).  Usage: coop_host_check <blob.bin> [cases]
 #include <math.h>
 #include <stdint.h>
@@ -18,43 +19,6 @@ static inline double rsqrt(double x) { return 1.0 / sqrt(x); }
 static inline float __saturatef(float x) { return x < 0.f ? 0.f : x > 1.f ? 1.f : x; }
 #include "../../robotics-rl-srl_b200/csrc/kuka_device.cuh"
 #include "../../robotics-rl-srl_b200/csrc/kuka_coop.cuh"
-
-static bool fill(const double* d, size_t n, KukaParams& P) {
-    if (n < KM_HEADER_SIZE || (int)d[KM_H_NBODY] != KK_NB) return false;
-    memset(&P, 0, sizeof(P));
-    const double* sc = d + (int)d[KM_H_SCENE_OFF];
-    for (int i = 0; i < KK_NB; ++i) {
-        const double* r = d + (int)d[KM_H_BODY_OFF] + i * KM_BODY_STRIDE;
-        for (int a = 0; a < 3; ++a) { P.org[i][a] = (float)r[KM_B_ORIGIN + a]; P.axis[i][a] = (float)r[KM_B_AXIS + a]; P.com[i][a] = (float)r[KM_B_COM + a]; }
-        for (int a = 0; a < 9; ++a) P.rot[i][a] = (float)r[KM_B_ROT + a];
-        for (int a = 0; a < 6; ++a) P.Ic[i][a] = (float)r[KM_B_INERTIA + a];
-        P.mass[i] = (float)r[KM_B_MASS];
-        P.snap_q[i] = (float)r[KM_B_QINIT];
-    }
-    P.nsph = (int)d[KM_H_NSPHERE];
-    P.sph_min_body = KK_NB; P.sph_reach = 0.f;
-    for (int k = 0; k < P.nsph; ++k) {
-        const double* sp = d + (int)d[KM_H_SPHERE_OFF] + k * KM_SPHERE_STRIDE;
-        P.sph_body[k] = (int)sp[KM_S_BODY]; P.sph_r[k] = (float)sp[KM_S_RADIUS];
-        for (int a = 0; a < 3; ++a) P.sph_c[k][a] = (float)sp[KM_S_CENTER + a];
-        if (P.sph_body[k] < P.sph_min_body) P.sph_min_body = P.sph_body[k];
-        const float reach = sqrtf(P.sph_c[k][0] * P.sph_c[k][0] + P.sph_c[k][1] * P.sph_c[k][1] + P.sph_c[k][2] * P.sph_c[k][2]) + P.sph_r[k];
-        if (reach > P.sph_reach) P.sph_reach = reach * 1.0001f;
-    }
-    for (int a = 0; a < 3; ++a) { P.base[a] = (float)sc[KM_SC_BASE_POS + a]; P.btn_base[a] = (float)sc[KM_SC_BUTTON_BASE + a]; }
-    P.gz = (float)sc[KM_SC_GRAVITY_Z]; P.dt = 1.f / 240.f; P.inv_dt = 240.f;
-    P.table_z = (float)sc[KM_SC_TABLE_TOP_Z]; P.txmin = (float)sc[KM_SC_TABLE_XMIN]; P.txmax = (float)sc[KM_SC_TABLE_XMAX];
-    P.tymin = (float)sc[KM_SC_TABLE_YMIN]; P.tymax = (float)sc[KM_SC_TABLE_YMAX];
-    P.glider_z = (float)sc[KM_SC_GLIDER_Z];
-    P.btn_minv = (float)(1.0 / sc[KM_SC_BUTTON_MASS]);
-    P.disc_r = (float)sc[KM_SC_DISC_RADIUS]; P.disc_z0 = (float)sc[KM_SC_DISC_Z0]; P.disc_z1 = (float)sc[KM_SC_DISC_Z1];
-    P.stack_r = (float)sc[KM_SC_STACK_RADIUS]; P.stack_top = (float)sc[KM_SC_STACK_TOP];
-    P.cdist = (float)sc[KM_SC_CONTACT_DIST]; P.erp = (float)sc[KM_SC_ERP];
-    P.kl = (float)sc[KM_SC_LIN_DAMPING]; P.ka = (float)sc[KM_SC_ANG_DAMPING];
-    P.max_contacts = (int)sc[KM_SC_MAX_CONTACTS];
-    if (P.max_contacts > KK_MAXC) P.max_contacts = KK_MAXC;
-    return true;
-}
 
 static double urand() { return rand() / (double)RAND_MAX; }
 static double g_max_rel[16];
@@ -75,14 +39,14 @@ static void run_cases(const KukaParams& P0, int cases) {
         e.qb = (float)(0.01 * urand()); e.qb2 = (float)(0.01 * urand());
         e.bbx = P.btn_base[0]; e.bby = P.btn_base[1]; e.bbz = P.btn_base[2]; e.bb2x = P.btn_base[0]; e.bb2y = -P.btn_base[1] - 0.25f;
         KukaKin k; KukaContacts ct; memset(&ct, 0, sizeof(ct));
-        kuka_fk<true, TWOB>(P, e, k, ct);
+        kuka_fk<TWOB>(P, e, k, ct);
         if (cs % 3) {
             // put the table / the button right under the lowest collision sphere so that the contact code runs
             float zlow = 1e30f; int blow = 0;
             for (int sidx = 0; sidx < P.nsph; ++sidx) { const int b = P.sph_body[sidx]; if (k.p[b].z < zlow) { zlow = k.p[b].z; blow = b; } }
             if (cs % 3 == 1) P.table_z = zlow - 0.03f - (float)(0.02 * urand());
             else { e.bbx = k.p[blow].x + (float)(0.02 * (urand() - 0.5)); e.bby = k.p[blow].y; e.bbz = zlow - 0.06f - P.glider_z - P.disc_z1 + (float)(0.02 * urand()); P.table_z = e.bbz - 0.5f; }
-            kuka_fk<true, TWOB>(P, e, k, ct);
+            kuka_fk<TWOB>(P, e, k, ct);
         }
         // ---- four-lane path ----
         kc_fill_const(P, tab.data(), 0, 1);
@@ -173,8 +137,8 @@ int main(int argc, char** argv) {
     std::vector<double> blob(1 << 16);
     const size_t n = fread(blob.data(), sizeof(double), blob.size(), f);
     fclose(f);
-    KukaParams P;
-    if (!fill(blob.data(), n, P)) { printf("bad blob\n"); return 2; }
+    KukaParams P;   // the model part of the library's parameter block, at the blob's own time step
+    if (const char* err = kuka_params_from_blob(blob.data(), n * sizeof(double), 0.0, P)) { printf("%s\n", err); return 2; }
     const int cases = argc > 2 ? atoi(argv[2]) : 300;
     srand(12345);
     run_cases<false>(P, cases);
