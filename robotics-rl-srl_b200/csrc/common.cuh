@@ -42,7 +42,6 @@ struct srl_sim {
     int max_steps;
     MobileDev mob;      // current state
     MobileDev mob_alt;  // the other half of the double buffer (rollouts write here, then swap)
-    int mobile_block;   // CTA-size override (0 = heuristic)
     KukaDev* kuka;
     KukaNext* kuka_next; // next-episode records, only with srl_cfg.prefetch_resets (nullptr: off)
     cudaEvent_t pf_ev;  // end of the last bulk record fill (srl_sim_prefetch_resets); the next rollout launch waits for it
@@ -63,7 +62,6 @@ struct srl_sim {
     float* render_prims; // [N][SRL_MAX_PRIMS][16] scene primitives of the last srl_sim_render (allocated on first use)
     float* render_prep;  // same shape: their per-camera prepared forms (render_core.h SrlPrep)
     int* render_counts;
-    bool host_zero_copy; // single-chunk rollouts store obs / reward / done straight into pinned, device-mapped host buffers (opt-in: SRL_HOST_ZEROCOPY=1)
 };
 
 static inline bool srl_is_mobile(int kind) { return kind >= SRL_ENV_MOBILE && kind <= SRL_ENV_MOBILE_LINE_TARGET; }

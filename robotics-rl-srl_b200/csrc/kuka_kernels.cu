@@ -757,9 +757,8 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
     const bool records = s->cfg.prefetch_resets && s->auto_reset && !d->P.two_buttons && !d->P.action_joints;
     if (auto_epw && records && (epw == 8 || epw == 32)) epw -= 1;
     d->epw = epw;
-    // four lanes per env while a warp carries at most 8 envs (the whole batch still fits one warp per scheduler); SRL_KUKA_COOP=0 / 1 overrides
+    // four lanes per env while a warp carries at most 8 envs (the whole batch still fits one warp per scheduler)
     d->coop = epw <= 8 ? 1 : 0;
-    if (const char* co = getenv("SRL_KUKA_COOP")) d->coop = (atoi(co) != 0 && epw <= 8) ? 1 : 0;
     // the 500 settle steps of reset(), once
     float* snap = nullptr;
     SRL_CUDA_OK(cudaMalloc(&snap, 32 * sizeof(float)));

@@ -176,15 +176,8 @@ constexpr double S_THR_04 = 0x1.47ae147ae147cp-3;
 //  * pass 2 turns those into distance, reward, observation and the HBM stores; its steps are independent;
 //  * nothing per-step is spent on episode bookkeeping: the step counter, `done`, the episode length follow from t, and
 //    the unshaped episode return is an integer sum (rewards are -1 / 0 / 1: the float64 accumulation is exact either way).
-#ifndef MOBILE_RING
-#define MOBILE_RING 4               // chunks of actions in the shared-memory ring (MOBILE_RING - 1 in flight ahead of the one being stepped)
-#endif
-#ifndef MOBILE_TABLE_DECODE
-#define MOBILE_TABLE_DECODE 1       // discrete action -> (dx, dy) through a 4-entry shared-memory table (one LDS.128) instead of 8 integer instructions
-#endif
-#ifndef MOBILE_PF
-#define MOBILE_PF 8                 // steps per chunk (8192 envs x 1024 steps: 8 was faster than 2 or 4)
-#endif
+constexpr int MOBILE_RING = 4;      // chunks of actions in the shared-memory ring (MOBILE_RING - 1 in flight ahead of the one being stepped; 4 was faster than 3 or 6)
+constexpr int MOBILE_PF = 8;        // steps per chunk (8192 envs x 1024 steps: 8 was faster than 2 or 4)
 
 template <bool DISCRETE, bool NOISE, int NS>
 struct ActionChunk {
@@ -253,8 +246,9 @@ __device__ __forceinline__ void step_chunk(MobileEnvRegs& e, SegmentAcc& acc, co
             // dx = [-dv, dv, 0, 0][a], dy = [0, 0, -dv, dv][a] (:242-243; 1D_env.py:115), branch-free: even actions flip the
             // sign bit, the axis that does not move gets +0.0
             const int a = cur.a[DISCRETE ? k : 0];
-            if (MOBILE_TABLE_DECODE && FAST && KIND != SRL_ENV_MOBILE_1D) {
-                // the four (dx, dy) pairs of the constant dv = DELTA_POS; `a & 3` is Python's list index for a in [-4, 3]
+            if (FAST && KIND != SRL_ENV_MOBILE_1D) {
+                // the four (dx, dy) pairs of the constant dv = DELTA_POS (one LDS.128 instead of 8 integer instructions);
+                // `a & 3` is Python's list index for a in [-4, 3]
                 const double2 d = delta_table[a & 3];
                 ax = d.x; ay = d.y;
             } else {
@@ -356,7 +350,7 @@ __global__ void __launch_bounds__(128) mobile_rollout_kernel(MobileDev in, Mobil
                                                              int max_steps, uint64_t seed, uint64_t env_offset) {
     // dx = [-dv, dv, 0, 0][a], dy = [0, 0, -dv, dv][a] (mobile_robot_env.py:242-243) for the constant dv of the FAST instantiation
     __shared__ double2 s_delta[4];
-    if (MOBILE_TABLE_DECODE && FAST && DISCRETE && KIND != SRL_ENV_MOBILE_1D) {
+    if (FAST && DISCRETE && KIND != SRL_ENV_MOBILE_1D) {
         if (threadIdx.x < 4) s_delta[threadIdx.x] = threadIdx.x < 2 ? make_double2(threadIdx.x ? DELTA_POS : -DELTA_POS, 0.0)
                                                                      : make_double2(0.0, threadIdx.x == 3 ? DELTA_POS : -DELTA_POS);
         __syncthreads();   // before any thread leaves
@@ -481,8 +475,7 @@ int launch_rollout_variant(srl_sim* s, int T, const void* actions, const float* 
     const int nseg = s->auto_reset ? (int)(1 + ((long long)T - 1 + per - 1) / per) : 1;
     // one warp per CTA while the whole launch is a few warps per SM: spreads the (latency-bound) warps over all SMs
     const long long warps = (long long)nseg * ((s->n + 31) / 32);
-    int block = warps <= (long long)s->sms * 4 ? 32 : 128;
-    if (s->mobile_block > 0) block = s->mobile_block;
+    const int block = warps <= (long long)s->sms * 4 ? 32 : 128;
     const dim3 grid((unsigned)((s->n + block - 1) / block), (unsigned)nseg);
     const size_t ring_bytes = GEN ? 0 : (size_t)MOBILE_RING * MOBILE_PF * 128 * (DISCRETE ? sizeof(int32_t) : sizeof(float2));   // rows of 128 lanes whatever the CTA size
     mobile_rollout_kernel<KIND, DISCRETE, GEN, SHAPED, FAST><<<grid, block, ring_bytes, st>>>(s->mob, s->mob_alt, s->n, T, actions, noise, obs, rew, done, ep_ret, ep_len,
@@ -510,8 +503,14 @@ int launch_rollout_kind(srl_sim* s, int T, const void* actions, const float* noi
     if (s->cfg.is_discrete)
         return actions ? launch_rollout_gen<KIND, true, false>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st)
                        : launch_rollout_gen<KIND, true, true>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st);
-    return actions ? launch_rollout_gen<KIND, false, false>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st)
-                   : launch_rollout_gen<KIND, false, true>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st);
+    // continuous actions exist for the 2-D kinds only (srl_sim_create rejects them for the others): no kernels for the rest
+    if constexpr (KIND == SRL_ENV_MOBILE || KIND == SRL_ENV_MOBILE_LINE_TARGET)
+        return actions ? launch_rollout_gen<KIND, false, false>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st)
+                       : launch_rollout_gen<KIND, false, true>(s, T, actions, noise, obs, rew, done, ep_ret, ep_len, st);
+    else {
+        srl_set_error("rollout: env kind %d has no continuous actions", KIND);
+        return 1;
+    }
 }
 
 }  // namespace
@@ -535,9 +534,6 @@ int mobile_alloc(srl_sim* s) {
     const size_t N = (size_t)s->n;
     if (mobile_alloc_one(s->mob, N)) return 1;
     if (mobile_alloc_one(s->mob_alt, N)) return 1;
-    const char* blk = getenv("SRL_MOBILE_BLOCK");   // CTA-size override for A/B measurements (32 / 64 / 128)
-    s->mobile_block = blk ? atoi(blk) : 0;
-    if (s->mobile_block != 32 && s->mobile_block != 64 && s->mobile_block != 128) s->mobile_block = 0;
     return 0;
 }
 

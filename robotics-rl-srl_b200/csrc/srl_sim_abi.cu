@@ -51,18 +51,8 @@ int ensure_host_pipe(srl_sim* s) {
     for (int k = 0; k < 2 * SRL_HOST_MAX_CHUNKS; ++k) SRL_CUDA_OK(cudaEventCreateWithFlags(&s->host_ev[k], cudaEventDisableTiming));
     const char* env = getenv("SRL_HOST_CHUNKS");
     s->host_chunks = env ? atoi(env) : 0;
-    const char* zc = getenv("SRL_HOST_ZEROCOPY");
-    s->host_zero_copy = zc && atoi(zc) != 0;   // opt-in: it did not pay where it was measured (see srl_sim_rollout_host)
     s->host_pipe_ready = true;
     return 0;
-}
-
-// Device-side alias of a pinned, device-mapped host buffer (cudaHostAlloc / cudaHostRegister memory under UVA), or nullptr for
-// pageable memory -- the kernel can then store its outputs straight into the caller's buffer over PCIe.
-char* mapped_host_alias(const void* p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
-    return (a.type == cudaMemoryTypeHost && a.devicePointer) ? (char*)a.devicePointer : nullptr;
 }
 
 int launch_rollout(srl_sim* s, int T, const void* actions, const float* noise, float* obs, float* rew, uint8_t* done,
@@ -227,22 +217,15 @@ int srl_sim_rollout_host(srl_sim* s, int T, const void* actions, const float* no
     if (chunks < 1) chunks = 1;
     if (chunks > SRL_HOST_MAX_CHUNKS) chunks = SRL_HOST_MAX_CHUNKS;
     if (chunks > T) chunks = T;
-    // Optional (SRL_HOST_ZEROCOPY=1): when the caller's output buffers are pinned and device-mapped, an unsplit rollout can store obs /
-    // reward / done STRAIGHT into them (posted PCIe writes) instead of staging them in HBM and copying them out afterwards.  Measured with
-    // the 4096-env x 128-step Kuka rollout, end to end it was no faster than staged (within run-to-run noise)
-    // -- the device->host copy it removes is paid back by the kernel draining its sysmem stores -- so the staged path stays the default.
-    char *z_obs = nullptr, *z_rew = nullptr, *z_done = nullptr;
-    if (chunks == 1 && s->host_zero_copy) {
-        if (obs_out) z_obs = mapped_host_alias(obs_out);
-        if (rew_out) z_rew = mapped_host_alias(rew_out);
-        if (done_out) z_done = mapped_host_alias(done_out);
-    }
-    char *d_act = nullptr, *d_noise = nullptr, *d_obs = z_obs, *d_rew = z_rew, *d_done = z_done;
+    // Outputs are always staged in HBM and copied out, also into pinned host buffers: letting the kernel store straight into pinned,
+    // device-mapped buffers was measured no faster end to end with the 4096-env x 128-step Kuka rollout (the device->host copy it
+    // removes is paid back by the kernel draining its sysmem stores).
+    char *d_act = nullptr, *d_noise = nullptr, *d_obs = nullptr, *d_rew = nullptr, *d_done = nullptr;
     if (actions) { if (ensure_stage(s, 0, T * act_step)) return 1; d_act = (char*)s->stage[0]; }
     if (noise) { if (ensure_stage(s, 1, T * noise_step)) return 1; d_noise = (char*)s->stage[1]; }
-    if (obs_out && !z_obs) { if (ensure_stage(s, 2, T * obs_step)) return 1; d_obs = (char*)s->stage[2]; }
-    if (rew_out && !z_rew) { if (ensure_stage(s, 3, T * rew_step)) return 1; d_rew = (char*)s->stage[3]; }
-    if (done_out && !z_done) { if (ensure_stage(s, 4, TN)) return 1; d_done = (char*)s->stage[4]; }
+    if (obs_out) { if (ensure_stage(s, 2, T * obs_step)) return 1; d_obs = (char*)s->stage[2]; }
+    if (rew_out) { if (ensure_stage(s, 3, T * rew_step)) return 1; d_rew = (char*)s->stage[3]; }
+    if (done_out) { if (ensure_stage(s, 4, TN)) return 1; d_done = (char*)s->stage[4]; }
     const int chunk_T = (T + chunks - 1) / chunks;
     cudaStream_t st_in = s->host_st[0], st_run = s->host_st[1], st_out = s->host_st[2];
     int c = 0;
@@ -262,9 +245,9 @@ int srl_sim_rollout_host(srl_sim* s, int T, const void* actions, const float* no
         if (rc) { cudaDeviceSynchronize(); return rc; }
         SRL_CUDA_OK(cudaEventRecord(s->host_ev[2 * c + 1], st_run));
         SRL_CUDA_OK(cudaStreamWaitEvent(st_out, s->host_ev[2 * c + 1], 0));
-        if (obs_out && !z_obs) SRL_CUDA_OK(cudaMemcpyAsync((char*)obs_out + t0 * obs_step, d_obs + t0 * obs_step, tc * obs_step, cudaMemcpyDeviceToHost, st_out));
-        if (rew_out && !z_rew) SRL_CUDA_OK(cudaMemcpyAsync((char*)rew_out + t0 * rew_step, d_rew + t0 * rew_step, tc * rew_step, cudaMemcpyDeviceToHost, st_out));
-        if (done_out && !z_done) SRL_CUDA_OK(cudaMemcpyAsync((char*)done_out + t0 * done_step, d_done + t0 * done_step, tc * done_step, cudaMemcpyDeviceToHost, st_out));
+        if (obs_out) SRL_CUDA_OK(cudaMemcpyAsync((char*)obs_out + t0 * obs_step, d_obs + t0 * obs_step, tc * obs_step, cudaMemcpyDeviceToHost, st_out));
+        if (rew_out) SRL_CUDA_OK(cudaMemcpyAsync((char*)rew_out + t0 * rew_step, d_rew + t0 * rew_step, tc * rew_step, cudaMemcpyDeviceToHost, st_out));
+        if (done_out) SRL_CUDA_OK(cudaMemcpyAsync((char*)done_out + t0 * done_step, d_done + t0 * done_step, tc * done_step, cudaMemcpyDeviceToHost, st_out));
     }
     SRL_CUDA_OK(cudaStreamSynchronize(st_run));   // the state update is complete even when no output was requested
     SRL_CUDA_OK(cudaStreamSynchronize(st_out));
