@@ -109,9 +109,15 @@ enum srl_state_field {
     SRL_F_BUTTON_BASE   = 10, /* f64[N,3] Kuka: button base link origin (x, y, z)              */
     SRL_F_TWO_BUTTON    = 11, /* f64[N,8] Kuka2Button (read-only): n_contacts[0], n_contacts[1], goal_id, second button base x y z,
                                  second glider q, qd (kuka_2button_gym_env.py:34,40-43)          */
-    SRL_F_NEXT_RECORD   = 12  /* i32[N,3] Kuka with srl_cfg.prefetch_resets (read-only, CUDA library): next-episode record
+    SRL_F_NEXT_RECORD   = 12, /* i32[N,3] Kuka with srl_cfg.prefetch_resets (read-only, CUDA library): next-episode record
                                  complete (0/1), random reset micro-steps applied to an incomplete record (0-4), episode index
                                  the record is for; all zero / -1 without the feature                         */
+    SRL_F_DISTRACTORS   = 13, /* f64[N,11,9] KukaRandButton distractor bodies (read-only): position xyz, orientation quaternion
+                                 xyz w, body type (0 duck_vhacd, 1 lego, 2 cube_small, 3 sphere_small), present (0/1); slots 0-9
+                                 are the 10 placements of reset() (absent inside the square around the button), slot 10 the
+                                 kicked sphere; all zero without srl_sim_set_distractors                       */
+    SRL_F_DISTRACTOR_TOUCH = 14 /* i32[N,2] (read-only) bit k set: distractor slot k touched another body / the arm since its
+                                 placement                                                                     */
 };
 
 int srl_sim_abi_version(void);
@@ -183,6 +189,16 @@ int srl_sim_rollout_host(srl_sim* sim, int T, const void* actions, const float* 
  * without the feature.  Reference: the reset() a SubprocVecEnv worker runs between two steps
  * (kuka_button_gym_env.py:214-281 via rl_baselines/utils.py:216-220). */
 int srl_sim_prefetch_resets(srl_sim* sim, void* stream);
+
+/* Opt-in for SRL_ENV_KUKA_RAND_BUTTON: simulate the reference's distractor objects (kuka_rand_button_gym_env.py:58-68,117-127) --
+ * up to 10 objects dropped at random positions around the button and a small sphere that is kicked at env step 10.  The bodies are
+ * free rigid bodies pushed by the arm, the button and the table, and by each other; they never push back, so observations, rewards,
+ * done flags and episode statistics are the same bytes with and without them.  `assets_blob` = f64[4][32] (srl_sim/model.py
+ * distractor_blob; layout in csrc/distractor_core.h).  Valid only between srl_sim_create and the first reset, and not together with
+ * srl_cfg.prefetch_resets.  With the bodies on, `reset_draws` rows are 48 wide: the 18 Kuka values, the 10 placements (x, y) as
+ * final positions and the 10 object types (0-2); NULL = all from the env's counter-based stream.  The object types and the kick
+ * direction come from the env's stream too (the reference draws them from the global, unseeded np.random).  State: SRL_F_DISTRACTORS. */
+int srl_sim_set_distractors(srl_sim* sim, const void* assets_blob, size_t bytes);
 
 /* Image observations (`srl_model = "raw_pixels"`): what the reference obtains per env from PyBullet's TinyRenderer in render(mode='rgb_array')
  * (environments/kuka_gym/kuka_button_gym_env.py:370-420, environments/mobile_robot/mobile_robot_env.py:287-334).  The camera is given the way

@@ -28,6 +28,7 @@ struct MobileDev {
 
 struct KukaDev;   // kuka_kernels.cu
 struct KukaNext;
+struct DistDev;
 
 #define SRL_HOST_MAX_CHUNKS 16
 
@@ -44,6 +45,9 @@ struct srl_sim {
     MobileDev mob_alt;  // the other half of the double buffer (rollouts write here, then swap)
     KukaDev* kuka;
     KukaNext* kuka_next; // next-episode records, only with srl_cfg.prefetch_resets (nullptr: off)
+    DistDev* dist;      // KukaRandButton distractor bodies, only after srl_sim_set_distractors (nullptr: off)
+    float kuka_q0[12];  // the initial joint vector the settle starts from
+    bool kuka_started;  // a reset / step / rollout has been issued
     cudaEvent_t pf_ev;  // end of the last bulk record fill (srl_sim_prefetch_resets); the next rollout launch waits for it
     bool pf_pending;
     cudaEvent_t roll_ev; // end of the last rollout launch of a handle with records; a bulk fill waits for it
@@ -88,5 +92,6 @@ int kuka_launch_rollout(srl_sim* s, int T, const void* actions, const float* noi
                         uint8_t* done, float* ep_ret, int32_t* ep_len, cudaStream_t st);
 int kuka_launch_prefetch(srl_sim* s, cudaStream_t st);
 int kuka_render_prims(srl_sim* s, float* prims, int* counts, cudaStream_t st);   // [N][SRL_MAX_PRIMS][16] primitive list of every env's scene
+int kuka_set_distractors(srl_sim* s, const void* blob, size_t bytes);
 int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes);
 int kuka_set_state(srl_sim* s, int field, const void* src, size_t bytes);

@@ -262,6 +262,13 @@ int srl_sim_render(srl_sim* s, const srl_camera* camera, int width, int height, 
     return render_launch(s, camera, width, height, rgb_out, (cudaStream_t)stream);
 }
 
+int srl_sim_set_distractors(srl_sim* s, const void* assets_blob, size_t bytes) {
+    if (!s) { srl_set_error("set_distractors: null handle"); return 1; }
+    if (!srl_is_kuka(s->kind)) { srl_set_error("set_distractors: only KukaRandButtonGymEnv-v0 has distractor bodies"); return 1; }
+    DeviceGuard guard(s->device);
+    return kuka_set_distractors(s, assets_blob, bytes);
+}
+
 int srl_sim_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
     if (!s || !dst) { srl_set_error("get_state: null argument"); return 1; }
     DeviceGuard guard(s->device);

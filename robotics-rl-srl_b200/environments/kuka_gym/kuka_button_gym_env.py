@@ -147,6 +147,8 @@ class KukaButtonGymEnv(SRLGymEnv):
             self.saver = EpisodeSaver(name, max_distance, state_dim, globals_=getGlobals(), relative_pos=RELATIVE_POS,
                                       learn_states=learn_states, path=save_path)
 
+        if _.get("distractors", False):
+            raise ValueError("distractors=True is only available for KukaRandButtonGymEnv-v0 (got %s)" % self._ENV_ID)
         self._backend = default_backend(device)
         self._sim = self._backend.make_sim(self._ENV_ID, 1, seed=0, model_blob=load_kuka_scene().blob,
                                            is_discrete=is_discrete, random_target=random_target, force_down=force_down,

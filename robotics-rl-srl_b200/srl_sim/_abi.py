@@ -32,17 +32,19 @@ ENV_KINDS = {
 
 # enum srl_state_field
 F_ROBOT_POS, F_TARGET_POS, F_STEP_COUNTER, F_JOINT_POS, F_JOINT_VEL, F_EE_CMD, F_EE_POS, \
-    F_BUTTON_GLIDER, F_COUNTERS, F_EPISODE_STATS, F_BUTTON_BASE, F_TWO_BUTTON, F_NEXT_RECORD = range(13)
+    F_BUTTON_GLIDER, F_COUNTERS, F_EPISODE_STATS, F_BUTTON_BASE, F_TWO_BUTTON, F_NEXT_RECORD, F_DISTRACTORS, F_DISTRACTOR_TOUCH = range(15)
 
 _FIELD_SPEC = {
     F_ROBOT_POS: (np.float64, 3), F_TARGET_POS: (np.float64, 3), F_STEP_COUNTER: (np.int32, 1),
     F_JOINT_POS: (np.float64, 12), F_JOINT_VEL: (np.float64, 12), F_EE_CMD: (np.float64, 3),
     F_EE_POS: (np.float64, 3), F_BUTTON_GLIDER: (np.float64, 2), F_COUNTERS: (np.int32, 4),
     F_EPISODE_STATS: (np.float64, 2), F_BUTTON_BASE: (np.float64, 3), F_TWO_BUTTON: (np.float64, 8), F_NEXT_RECORD: (np.int32, 3),
+    F_DISTRACTORS: (np.float64, 11 * 9), F_DISTRACTOR_TOUCH: (np.int32, 2),
 }
 
 MOBILE_RESET_DRAWS = 6
 KUKA_RESET_DRAWS = 18
+KUKA_DISTRACTOR_RESET_DRAWS = 48   # with srl_sim_set_distractors: + 10 placements (x, y) + 10 object types
 
 
 class SrlCfg(Structure):
@@ -91,7 +93,12 @@ _EXPORTS = [
     ("srl_sim_destroy", None, [c_void_p]),
 ]
 
-EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS]
+# opt-in features that only the CUDA library implements (the CPU oracle does not): bound when the library exports them
+_OPTIONAL_EXPORTS = [
+    ("srl_sim_set_distractors", c_int, [c_void_p, c_void_p, c_size_t]),
+]
+
+EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS + _OPTIONAL_EXPORTS]   # everything include/srl_sim.h declares
 
 
 def _ptr(x):
@@ -126,6 +133,13 @@ class SimLibrary(object):
                 raise SimError("%s does not export %s" % (self.path, name))
             fn.restype = restype
             fn.argtypes = argtypes
+        self.optional = set()
+        for name, restype, argtypes in _OPTIONAL_EXPORTS:
+            fn = getattr(self.lib, name, None)
+            if fn is not None:
+                fn.restype = restype
+                fn.argtypes = argtypes
+                self.optional.add(name)
         v = self.lib.srl_sim_abi_version()
         if v != ABI_VERSION:
             raise SimError("ABI version mismatch: library %d, binding %d" % (v, ABI_VERSION))
@@ -231,6 +245,15 @@ class Sim(object):
         """One ``width`` x ``height`` RGB frame per env into ``rgb_out`` (u8[N, H, W, 3]); ``cam`` is an ``srl_sim.render.SrlCamera``."""
         rc = self._lib.srl_sim_render(self.handle, ctypes.byref(cam), int(width), int(height), _ptr(rgb_out), stream)
         self.library.check(rc, "srl_sim_render")
+
+    def set_distractors(self, assets_blob):
+        """KukaRandButtonGymEnv-v0 only, before the first reset: simulate the distractor bodies (``srl_sim.model.distractor_blob``).
+        Observations, rewards and done flags do not change; the bodies' state is ``get_state(F_DISTRACTORS)``."""
+        if "srl_sim_set_distractors" not in self.library.optional:
+            raise SimError("%s does not implement distractor bodies" % self.library.path)
+        self._dist_blob = np.ascontiguousarray(assets_blob, dtype=np.float64)
+        rc = self._lib.srl_sim_set_distractors(self.handle, self._dist_blob.ctypes.data, self._dist_blob.nbytes)
+        self.library.check(rc, "srl_sim_set_distractors")
 
     # -- state access ------------------------------------------------------------------------
     def get_state(self, field):

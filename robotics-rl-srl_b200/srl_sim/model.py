@@ -401,3 +401,58 @@ def load_kuka_scene():
     if _default_scene is None:
         _default_scene = KukaScene()
     return _default_scene
+
+
+# ---- KukaRandButtonGymEnv distractor bodies (csrc/distractor_core.h) ------------------------------------------------------------
+# The reference loads pybullet_data's duck_vhacd.urdf, lego/lego.urdf, cube_small.urdf and sphere_small.urdf
+# (kuka_rand_button_gym_env.py:58,68); neither the meshes nor the URDFs are available here.  The values below are RECALLED from
+# pybullet_data (mass, size, colour) and unpinned like the rest of the Kuka restatement (SURVEY Appendix C); the collision geometry
+# is a compound of at most 4 spheres per body, the way the arm's fingers are modelled.  Inertias are those of the solid shapes.
+# name: (mass kg, lateral friction, [(cx, cy, cz, r)] in the link frame = COM frame, half extents for drawing, rgb, 0 box / 1 sphere)
+DISTRACTOR_TYPES = ("duck_vhacd", "lego", "cube_small", "sphere_small")
+_DISTRACTOR_ASSETS = {
+    # a ~0.1 m duck: body and head
+    "duck_vhacd": (0.1, 0.5, [(-0.01, 0.0, -0.005, 0.03), (0.025, 0.0, 0.035, 0.02), (-0.03, 0.0, 0.0, 0.025)],
+                   (0.045, 0.03, 0.04), (1.0, 0.85, 0.0), 0),
+    # a 2 x 2 brick, 32 x 32 x 19 mm: four spheres in a square (rests flat)
+    "lego": (0.05, 0.5, [(sx * 0.008, sy * 0.008, 0.0, 0.0095) for sx in (-1, 1) for sy in (-1, 1)],
+             (0.016, 0.016, 0.0095), (0.9, 0.1, 0.1), 0),
+    # a 5 cm cube: four spheres of radius s/4 on alternate corners of the inner cube (their hull reaches every face)
+    "cube_small": (0.1, 0.5, [(0.0125, 0.0125, 0.0125, 0.0125), (0.0125, -0.0125, -0.0125, 0.0125),
+                              (-0.0125, 0.0125, -0.0125, 0.0125), (-0.0125, -0.0125, 0.0125, 0.0125)],
+                   (0.025, 0.025, 0.025), (0.8, 0.8, 0.8), 0),
+    # a 3 cm ball
+    "sphere_small": (0.1, 0.5, [(0.0, 0.0, 0.0, 0.03)], (0.03, 0.03, 0.03), (0.3, 0.3, 0.9), 1),
+}
+
+
+def distractor_blob():
+    """f64[4][32] asset blob of srl_sim_set_distractors (layout: csrc/distractor_core.h, DC_A_*)."""
+    out = np.zeros((len(DISTRACTOR_TYPES), 32), np.float64)
+    for t, name in enumerate(DISTRACTOR_TYPES):
+        mass, mu, spheres, half, rgb, shape = _DISTRACTOR_ASSETS[name]
+        if shape == 1:
+            inertia = [0.4 * mass * half[0] ** 2] * 3
+        else:
+            a, b, c = (2 * h for h in half)
+            inertia = [mass / 12.0 * (b * b + c * c), mass / 12.0 * (a * a + c * c), mass / 12.0 * (a * a + b * b)]
+        row = out[t]
+        row[0] = mass
+        row[1:4] = inertia
+        row[4] = mu
+        row[5] = len(spheres)
+        for k, sph in enumerate(spheres):
+            row[6 + 4 * k:10 + 4 * k] = sph
+        row[22:25] = half
+        row[25:28] = rgb
+        row[28] = shape
+    return out.reshape(-1)
+
+
+def scene_constants(scene):
+    """Table top and button geometry of a loaded KukaScene, as the libraries read them from the blob."""
+    g = lambda name: float(scene.scene[KM[name]])   # noqa: E731
+    return dict(table_z=g("KM_SC_TABLE_TOP_Z"), txmin=g("KM_SC_TABLE_XMIN"), txmax=g("KM_SC_TABLE_XMAX"), tymin=g("KM_SC_TABLE_YMIN"),
+                tymax=g("KM_SC_TABLE_YMAX"), button_z=float(scene.scene[KM["KM_SC_BUTTON_BASE"] + 2]), glider_z=g("KM_SC_GLIDER_Z"),
+                disc_z0=g("KM_SC_DISC_Z0"), disc_z1=g("KM_SC_DISC_Z1"), disc_r=g("KM_SC_DISC_RADIUS"), stack_top=g("KM_SC_STACK_TOP"),
+                stack_r=g("KM_SC_STACK_RADIUS"))

@@ -59,6 +59,9 @@ class BatchedSRLVecEnv(object):
                 self._cams = [dict(_render.MOBILE_CAMERA, target=(2, 0, 0) if env_id == "MobileRobot1DGymEnv-v0" else (2, 2, 0))]
                 if env_kwargs.get("fpv", False):
                     raise NotImplementedError("fpv frames follow each robot: use the single-env classes (one camera per env)")
+        self.distractors = bool(env_kwargs.get("distractors", False))
+        if self.distractors and env_id != "KukaRandButtonGymEnv-v0":
+            raise ValueError("distractors=True is only available for KukaRandButtonGymEnv-v0 (got %r)" % env_id)
         self.srl_model = srl_model
         self.env_id = env_id
         self.num_envs = int(num_envs)
@@ -78,6 +81,10 @@ class BatchedSRLVecEnv(object):
             if k in env_kwargs:
                 cfg[k] = env_kwargs[k]
         self.sim = self.backend.make_sim(env_id, self.num_envs, seed=seed, model_blob=blob, **cfg)
+        if self.distractors:
+            # kuka_rand_button_gym_env.py:58-68: random objects around the button and a kicked sphere (one-way coupled: the arm's outputs do not change)
+            from .model import distractor_blob
+            self.sim.set_distractors(distractor_blob())
         self.is_discrete = bool(cfg["is_discrete"])
         D = self.sim.obs_dim
         # Kuka `joints` / `joints_position` states (kuka_button_gym_env.py:175-189): the 14 stored joint positions are the
