@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
+#include <atomic>
 #include "../../include/srl_sim.h"
 
 void srl_set_error(const char* fmt, ...);
@@ -17,6 +18,20 @@ void srl_set_error(const char* fmt, ...);
         }                                                                                   \
     } while (0)
 
+// Opt `Kernel` in to `bytes` (> 48 KB) of dynamic shared memory on the current device.  The attribute belongs to the device context,
+// so it is set once per kernel and device; a process with handles on several devices sets it on each.
+template <auto Kernel>
+cudaError_t srl_smem_opt_in(size_t bytes) {
+    static std::atomic<uint64_t> devices{0};   // bit d: set on device d (devices from 64 on: set at every call)
+    int dev = 0;
+    if (const cudaError_t e = cudaGetDevice(&dev)) return e;
+    const uint64_t bit = dev >= 0 && dev < 64 ? 1ull << dev : 0ull;
+    if (devices.load(std::memory_order_relaxed) & bit) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) devices.fetch_or(bit, std::memory_order_relaxed);
+    return e;
+}
+
 // ---- MobileRobot family: structure-of-arrays state in HBM, 16-byte records per field -----
 struct MobileDev {
     double2* pos;   // [N] robot_pos (x, y); z is identically 0 (mobile_robot_env.py:170)
@@ -26,9 +41,9 @@ struct MobileDev {
     double2* ep;    // [N] {running episode return, running episode length}
 };
 
-struct KukaDev;   // kuka_kernels.cu
-struct KukaNext;
-struct DistDev;
+struct KukaDev;   // kuka_state.cuh
+struct KukaNext;  // kuka_kernels.cu
+struct DistDev;   // distractor_kernels.cu
 
 #define SRL_HOST_MAX_CHUNKS 16
 
@@ -95,3 +110,10 @@ int kuka_render_prims(srl_sim* s, float* prims, int* counts, cudaStream_t st);  
 int kuka_set_distractors(srl_sim* s, const void* blob, size_t bytes);
 int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes);
 int kuka_set_state(srl_sim* s, int field, const void* src, size_t bytes);
+
+// ---- KukaRandButton's distractor bodies (distractor_kernels.cu), driven by the Kuka launchers ----------------------------------
+int dist_alloc(srl_sim* s, const void* blob, size_t bytes, float4** settle);   // checks, assets, buffers; *settle: room for the arm's settle trace
+int dist_trace(srl_sim* s, size_t steps, cudaStream_t st, float4** trace, int** trace_len);   // trace buffers for <= `steps` micro-steps per env
+int dist_advance(srl_sim* s, const double* draws, cudaStream_t st);   // distractor_kernel through the micro-steps of the last traced launch
+void dist_free(srl_sim* s);
+int dist_get_state(srl_sim* s, int field, void* dst, size_t bytes);   // SRL_F_DISTRACTORS, SRL_F_DISTRACTOR_TOUCH

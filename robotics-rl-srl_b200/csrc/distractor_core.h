@@ -1,6 +1,6 @@
 // KukaRandButtonGymEnv's distractor bodies (kuka_rand_button_gym_env.py:58-68,117-127): up to 10 objects dropped on the table
 // plus the small sphere that is kicked at env step 10.  One header for both sides: the CUDA library instantiates it in float
-// (distractor_kernel, kuka_kernels.cu) and the float64 CPU checker (distractor_ref.cpp) in double.
+// (distractor_kernel, distractor_kernels.cu) and the float64 CPU checker (distractor_ref.cpp) in double.
 //
 // Model (DESIGN.md section 4, "Distractor bodies"):
 //   * free 6-DoF bodies, gravity -g along z, time step dt; no damping, no sleeping, no rolling friction;

@@ -121,6 +121,28 @@ KK_DEV void sphere_cylinder(f3 s, float r, float cx, float cy, float z0, float z
     dist = d - r;
 }
 
+// World rotation and origin of every body's joint frame at joint vector q: the chain of kuka_fk with every rotation kept, for the code
+// off the hot path (srl_sim_render's scene primitives, the arm as the distractor bodies see it)
+KK_DEV void kuka_world_frames(const KukaParams& P, const float* q, float (&Rb)[KK_NB][9], f3 (&pb)[KK_NB]) {
+    float R[9] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f}, R7[9]; f3 p = mk3(P.base[0], P.base[1], P.base[2]), p7 = p;
+    for (int t = 0; t < 9; ++t) R7[t] = R[t];
+    for (int b = 0; b < KK_NB; ++b) {
+        if (b == 10) { for (int t = 0; t < 9; ++t) R[t] = R7[t]; p = p7; }   // the second finger restarts from the gripper base
+        const float ox = P.org[b][0], oy = P.org[b][1], oz = P.org[b][2];
+        p = mk3(p.x + R[0] * ox + R[1] * oy + R[2] * oz, p.y + R[3] * ox + R[4] * oy + R[5] * oz, p.z + R[6] * ox + R[7] * oy + R[8] * oz);
+        float sn, cs; sincosf(q[b], &sn, &cs);
+        const float t = 1.f - cs, ax = P.axis[b][0], ay = P.axis[b][1], az = P.axis[b][2];
+        const float Q[9] = {cs + t * ax * ax, t * ax * ay - sn * az, t * ax * az + sn * ay, t * ax * ay + sn * az, cs + t * ay * ay, t * ay * az - sn * ax,
+                            t * ax * az - sn * ay, t * ay * az + sn * ax, cs + t * az * az};
+        float B[9], Rn[9];
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) B[3 * r + c] = P.rot[b][3 * r] * Q[c] + P.rot[b][3 * r + 1] * Q[3 + c] + P.rot[b][3 * r + 2] * Q[6 + c];
+        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Rn[3 * r + c] = R[3 * r] * B[c] + R[3 * r + 1] * B[3 + c] + R[3 * r + 2] * B[6 + c];
+        for (int t2 = 0; t2 < 9; ++t2) { R[t2] = Rn[t2]; Rb[b][t2] = Rn[t2]; }
+        pb[b] = p;
+        if (b == 7) { for (int t2 = 0; t2 < 9; ++t2) R7[t2] = R[t2]; p7 = p; }
+    }
+}
+
 // Forward kinematics + link states + collision detection against table / button disc / button stack.
 //
 // CODE-SIZE NOTE (measured): this kernel runs ONE warp per scheduler, and everything outside the PGS sweep

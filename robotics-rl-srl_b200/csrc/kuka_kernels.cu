@@ -1,4 +1,4 @@
-// Kuka button-push family -- kernels and host launchers (sm_90a).
+// Kuka button-push family -- kernels and host launchers (sm_90a).  KukaRandButton's distractor bodies: distractor_kernels.cu.
 //
 // Replaces, for thousands of envs in lockstep, KukaButtonGymEnv.reset/step/step2/_reward/_termination
 // (environments/kuka_gym/kuka_button_gym_env.py:214-281,293-368,422-463), Kuka.applyAction
@@ -16,29 +16,9 @@
 #include <string.h>
 #include <vector>
 #include "common.cuh"
+#include "kuka_state.cuh"
 #include "kuka_device.cuh"
 #include "render_core.h"
-#include "distractor_core.h"
-
-// Per-env state in HBM, one 16-byte record per array: the live state (KukaDev) and the next-episode records (KukaNext) alike.
-struct KukaState {
-    float4* q[3];    // [N] joint positions  (12 floats as 3 x float4)
-    float4* qd[3];   // [N] joint velocities
-    float4* misc0;   // ee.x ee.y ee.z qb
-    float4* misc1;   // qdb btn_base.x btn_base.y ep_ret
-    float4* tgt;     // button_pos.xyz, button base z
-    float4* grip;    // gripper_pos.xyz, signed button speed
-    float4* eepos;   // link-6 origin xyz, moving button: low word of the float64 target y
-    int4*   cnt;     // counter, n_contacts, n_outside, terminated | cbutton << 1 | ctable << 2
-    int4*   cnt2;    // episode, total_steps, ep_len, moving button: high word of the float64 target y / two buttons: n_contacts[1]
-    float4* btn2;    // two buttons only: second glider q, qd, second button base x, y
-};
-
-struct KukaDev : KukaState {
-    KukaParams P;
-    int epw;         // live env slots per warp (lanes, or groups of 4 lanes when coop)
-    int coop;        // 1: four lanes per env (kuka_coop.cuh), epw <= 8
-};
 
 // "Next episode" records (opt-in, srl_cfg.prefetch_resets): the post-reset state of every env's NEXT episode -- a pure function of
 // (seed, global env index, episode index) -- produced ahead of time, so that a LOCKSTEP step whose env finishes an episode copies a
@@ -52,20 +32,6 @@ struct KukaDev : KukaState {
 // clean, but its long launches shared schedulers with 2-4 following step launches and doubled their duration.  A helper CTA on the
 // last SM worked too, but cannot serve enough records once an env takes 4 lanes.)
 // op = PREFETCH as a launch of its own (srl_sim_prefetch_resets) remains as the bulk fill after an explicit reset of all envs.
-// KukaRandButton's distractor bodies (opt-in, srl_sim_set_distractors; distractor_core.h).  The arm never feels them, so they are advanced
-// by a kernel of their own after every traced kuka_kernel launch: the trace holds, per env and micro-step, the arm configuration the
-// micro-step starts from and its kind (64 B: q[12], glider q, button base x y, tag).  Capacity: T (action_repeat + 5) micro-steps per env
-// -- at 4096 envs x 128 steps x (1 + 5) that is 201 MB.  The arm's 500 settle micro-steps are one fixed trajectory per handle (`settle`).
-struct DistDev {
-    float* body;         // [N][DC_NBODY][DC_B_WORDS]
-    uint32_t* touch;     // [N][2] bodies that touched another body / the arm since their placement (bit k = slot k)
-    float4* trace;       // [cap][4][N]
-    int* trace_len;      // [N] micro-steps of the last traced launch
-    float4* settle;      // [500][4] the arm's settle trajectory
-    size_t cap;          // micro-steps per env the trace holds
-    DcAssets<float> A;
-};
-
 struct KukaNext : KukaState {
     uint8_t* valid;     // [N] 1 = record complete and not yet consumed
     int32_t* episode;   // [N] episode index the record was produced for (a record for another episode is dropped)
@@ -215,14 +181,6 @@ KK_DEV void reset_end(const KukaParams& P, KukaEnv& e) {
 }
 
 enum { KUKA_OP_ROLLOUT = 0, KUKA_OP_RESET = 1, KUKA_OP_SETTLE = 2, KUKA_OP_PREFETCH = 3 };
-// trace tags of a micro-step (low 4 bits; the env's episode index above them): inside reset(), the first micro-step of a reset() (the
-// bodies are placed and settled before it), placement values supplied by the host, the step() that kicks the sphere
-enum { DT_RESET = 1, DT_FIRST = 2, DT_HOST_DRAWS = 4, DT_KICK = 8 };
-// reset_draws row width with distractor bodies: the 18 Kuka values, the 10 final placements (x, y) and the 10 object types
-constexpr int KUKA_DIST_DRAWS = 48;
-// Philox purposes of the bodies (philox.cuh: 0-10 are the simulator's, policy_core.h: 16 and up the policy's): 0x100-0x109 placement k,
-// 0x10A kick direction, 0x10B-0x10D object types
-enum { PHILOX_PURPOSE_DIST_PLACE = 0x100, PHILOX_PURPOSE_DIST_KICK = 0x10A, PHILOX_PURPOSE_DIST_TYPE = 0x10B /* 0x10B-0x10D */ };
 
 // ONE kernel for reset, lockstep step and fused T-step rollout.  Every thread runs a single micro-step loop
 //     forward kinematics + collision detection  ->  [finish the env step whose physics just ran: reward, done,
@@ -250,8 +208,8 @@ __device__ unsigned long long kk_timing[1 << 16];
 __device__ unsigned long long kk_phase[1 << 13][KK_NPH + 1];
 #endif
 // TRACE (KukaRandButton with distractor bodies only): every micro-step also writes the arm configuration it starts from and what kind
-// of micro-step it is to `trace` ([micro-step][4][N] float4, see DistDev), and each env its number of micro-steps to `trace_len`;
-// distractor_kernel then advances the bodies through the same micro-steps.  TRACE = false: the kernel is what it was before.
+// of micro-step it is to `trace` (layout: kuka_state.cuh), and each env its number of micro-steps to `trace_len`; distractor_kernel
+// (distractor_kernels.cu) then advances the bodies through the same micro-steps.  TRACE = false: the kernel is what it was before.
 template <bool JOINTS, bool TWOB, bool PREFETCH = false, bool COOP = false, bool TRACE = false>
 __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ KukaDev d, int n, int op, int T,
                                                        const void* __restrict__ actions, const float* __restrict__ noise,
@@ -655,29 +613,11 @@ __global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, floa
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const KukaParams& P = d.P;
-    KukaEnv e; KukaKin k; KukaContacts ct;
+    KukaEnv e;
     env_load<TWOB>(d, i, e);
     // world rotations are needed for the sphere centres: rerun the chain with the rotations kept (12 bodies, negligible next to the ray-casting)
     float Rb[KK_NB][9]; f3 pb[KK_NB];
-    {
-        float R[9] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f}, R7[9]; f3 p = mk3(P.base[0], P.base[1], P.base[2]), p7 = p;
-        for (int t = 0; t < 9; ++t) R7[t] = R[t];
-        for (int b = 0; b < KK_NB; ++b) {
-            if (b == 10) { for (int t = 0; t < 9; ++t) R[t] = R7[t]; p = p7; }
-            const float ox = P.org[b][0], oy = P.org[b][1], oz = P.org[b][2];
-            p = mk3(p.x + R[0] * ox + R[1] * oy + R[2] * oz, p.y + R[3] * ox + R[4] * oy + R[5] * oz, p.z + R[6] * ox + R[7] * oy + R[8] * oz);
-            float sn, cs; sincosf(e.q[b], &sn, &cs);
-            const float t = 1.f - cs, ax = P.axis[b][0], ay = P.axis[b][1], az = P.axis[b][2];
-            const float Q[9] = {cs + t * ax * ax, t * ax * ay - sn * az, t * ax * az + sn * ay, t * ax * ay + sn * az, cs + t * ay * ay, t * ay * az - sn * ax,
-                                t * ax * az - sn * ay, t * ay * az + sn * ax, cs + t * az * az};
-            float B[9], Rn[9];
-            for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) B[3 * r + c] = P.rot[b][3 * r] * Q[c] + P.rot[b][3 * r + 1] * Q[3 + c] + P.rot[b][3 * r + 2] * Q[6 + c];
-            for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Rn[3 * r + c] = R[3 * r] * B[c] + R[3 * r + 1] * B[3 + c] + R[3 * r + 2] * B[6 + c];
-            for (int t2 = 0; t2 < 9; ++t2) { R[t2] = Rn[t2]; Rb[b][t2] = Rn[t2]; }
-            pb[b] = p;
-            if (b == 7) { for (int t2 = 0; t2 < 9; ++t2) R7[t2] = R[t2]; p7 = p; }
-        }
-    }
+    kuka_world_frames(P, e.q, Rb, pb);
     float jp[KK_NB * 3], sph[KM_MAX_SPHERES * 4];
     for (int b = 0; b < KK_NB; ++b) { jp[3 * b] = pb[b].x; jp[3 * b + 1] = pb[b].y; jp[3 * b + 2] = pb[b].z; }
     int ns = 0;
@@ -698,161 +638,6 @@ __global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, floa
     K.two_buttons = TWOB ? 1 : 0;
     SrlPrim* out = reinterpret_cast<SrlPrim*>(prims + (size_t)i * SRL_MAX_PRIMS * SRL_PRIM_WORDS);
     counts[i] = srl_kuka_scene(K, jp, sph, ns, e.bbx, e.bby, e.bbz, e.qb, e.bb2x, e.bb2y, P.btn_base[2], e.qb2, out);
-    (void)k; (void)ct;
-}
-
-// world centres and radii of the arm's collision spheres at joint configuration q (the chain of kuka_prims_kernel)
-KK_DEV int arm_spheres(const KukaParams& P, const float* q, float* out) {
-    float Rb[KK_NB][9]; f3 pb[KK_NB];
-    float R[9] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f}, R7[9]; f3 p = mk3(P.base[0], P.base[1], P.base[2]), p7 = p;
-    for (int t = 0; t < 9; ++t) R7[t] = R[t];
-    for (int b = 0; b < KK_NB; ++b) {
-        if (b == 10) { for (int t = 0; t < 9; ++t) R[t] = R7[t]; p = p7; }
-        const float ox = P.org[b][0], oy = P.org[b][1], oz = P.org[b][2];
-        p = mk3(p.x + R[0] * ox + R[1] * oy + R[2] * oz, p.y + R[3] * ox + R[4] * oy + R[5] * oz, p.z + R[6] * ox + R[7] * oy + R[8] * oz);
-        float sn, cs; sincosf(q[b], &sn, &cs);
-        const float t = 1.f - cs, ax = P.axis[b][0], ay = P.axis[b][1], az = P.axis[b][2];
-        const float Q[9] = {cs + t * ax * ax, t * ax * ay - sn * az, t * ax * az + sn * ay, t * ax * ay + sn * az, cs + t * ay * ay, t * ay * az - sn * ax,
-                            t * ax * az - sn * ay, t * ay * az + sn * ax, cs + t * az * az};
-        float Bm[9], Rn[9];
-        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Bm[3 * r + c] = P.rot[b][3 * r] * Q[c] + P.rot[b][3 * r + 1] * Q[3 + c] + P.rot[b][3 * r + 2] * Q[6 + c];
-        for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) Rn[3 * r + c] = R[3 * r] * Bm[c] + R[3 * r + 1] * Bm[3 + c] + R[3 * r + 2] * Bm[6 + c];
-        for (int t2 = 0; t2 < 9; ++t2) { R[t2] = Rn[t2]; Rb[b][t2] = Rn[t2]; }
-        pb[b] = p;
-        if (b == 7) { for (int t2 = 0; t2 < 9; ++t2) R7[t2] = R[t2]; p7 = p; }
-    }
-    const int ns = P.nsph < DC_MAXARM ? P.nsph : DC_MAXARM;
-    for (int k = 0; k < ns; ++k) {
-        const int b = P.sph_body[k];
-        const float* Rk = Rb[b];
-        out[4 * k] = pb[b].x + Rk[0] * P.sph_c[k][0] + Rk[1] * P.sph_c[k][1] + Rk[2] * P.sph_c[k][2];
-        out[4 * k + 1] = pb[b].y + Rk[3] * P.sph_c[k][0] + Rk[4] * P.sph_c[k][1] + Rk[5] * P.sph_c[k][2];
-        out[4 * k + 2] = pb[b].z + Rk[6] * P.sph_c[k][0] + Rk[7] * P.sph_c[k][1] + Rk[8] * P.sph_c[k][2];
-        out[4 * k + 3] = P.sph_r[k];
-    }
-    return ns;
-}
-
-// the scene of one micro-step from a trace record: button base + disc at the glider q
-KK_DEV void dist_scene(const KukaParams& P, DcScene<float>& S, float qb, float bx, float by) {
-    S.bx = bx; S.by = by; S.bz = P.btn_base[2];
-    S.disc0 = S.bz + P.glider_z + qb + P.disc_z0; S.disc1 = S.bz + P.glider_z + qb + P.disc_z1;
-}
-
-// A group of 16 lanes per env (2 envs per warp) advances its bodies through the micro-steps the preceding traced kuka_kernel launch
-// recorded: lane k < 11 owns body k (prepare, adjacency, integrate), and the lowest lane of every island of bodies in contact runs that
-// island's rows and sweeps (distractor_core.h: the same arithmetic as the one-thread dc_step).  Body state and the per-micro-step work
-// arrays live in shared memory; a lane's contact rows in its own local memory.  At the first micro-step of a reset() the group places the
-// bodies (host values or the env's counter-based stream) and runs the 500 settle micro-steps against the arm's settle trajectory first.
-constexpr int DIST_LANES = 16, DIST_BLOCK = 128, DIST_ENVS_PER_BLOCK = DIST_BLOCK / DIST_LANES;
-struct DistShared {
-    float B[DC_NBODY * DC_B_WORDS];
-    DcWork<float> W;
-    uint32_t adj[DC_NBODY];
-};
-
-KK_DEV void dist_micro_step(const DcAssets<float>& A, const DcScene<float>& S, DistShared& sh, int u, unsigned gmask, const float* arm, int na,
-                            const float* kick, DcRow<float>* rows, DcTouch& touch) {
-    if (u < DC_NBODY) dc_prepare(A, sh.B, u, sh.W, kick, S);
-    __syncwarp(gmask);
-    if (u < DC_NBODY) sh.adj[u] = dc_adjacency(A, S, sh.B, sh.W, u);
-    __syncwarp(gmask);
-    int root[DC_NBODY];
-    uint32_t adj[DC_NBODY];
-    for (int k = 0; k < DC_NBODY; ++k) adj[k] = sh.adj[k];
-    dc_island_roots(adj, root);
-    if (u < DC_NBODY && root[u] == u && sh.B[u * DC_B_WORDS + DC_B_PRESENT] != 0.f) dc_island_solve(A, S, sh.B, sh.W, u, root, arm, na, rows, &touch);
-    __syncwarp(gmask);
-    if (u < DC_NBODY) dc_integrate(S, sh.B, u);
-    __syncwarp(gmask);
-}
-
-__global__ void __launch_bounds__(DIST_BLOCK) distractor_kernel(const __grid_constant__ KukaDev d, const __grid_constant__ DistDev g, int n,
-                                                                 const double* __restrict__ draws) {
-    __shared__ DistShared shared[DIST_ENVS_PER_BLOCK];
-    const int lane = threadIdx.x & 31, u = lane & (DIST_LANES - 1);
-    const unsigned gmask = 0xFFFFu << (lane & ~(DIST_LANES - 1));
-    const int slot = threadIdx.x / DIST_LANES;
-    const int i = blockIdx.x * DIST_ENVS_PER_BLOCK + slot;
-    if (i >= n) return;                      // whole groups leave together
-    const int len = g.trace_len[i];
-    if (len <= 0) return;
-    DistShared& sh = shared[slot];
-    const KukaParams& P = d.P;
-    const size_t N = (size_t)n;
-    const uint64_t genv = P.env_offset + (uint64_t)i;
-    float* const gb = g.body + (size_t)i * DC_NBODY * DC_B_WORDS;
-    for (int j = u; j < DC_NBODY * DC_B_WORDS; j += DIST_LANES) sh.B[j] = gb[j];
-    DcTouch touch = {0u, 0u};
-    DcScene<float> S;
-    S.table_z = P.table_z; S.txmin = P.txmin; S.txmax = P.txmax; S.tymin = P.tymin; S.tymax = P.tymax;
-    S.stack_top = P.stack_top; S.stack_r = P.stack_r; S.disc_r = P.disc_r;
-    S.dt = P.dt; S.g = 10.f; S.margin = P.cdist; S.iters = P.iters;   // setGravity(0, 0, -10) (:71)
-    DcRow<float> rows[3 * DC_MAXC];
-    float arm[DC_MAXARM * 4];
-    uint32_t clear = 0u;                     // lane 0: the touch masks were reset by a placement in this launch
-    __syncwarp(gmask);
-    for (int m = 0; m < len; ++m) {
-        const size_t base = (size_t)m * 4 * N + (size_t)i;
-        const float4 r0 = g.trace[base], r1 = g.trace[base + N], r2 = g.trace[base + 2 * N], r3 = g.trace[base + 3 * N];
-        const int tag = __float_as_int(r3.w);
-        const uint32_t episode = (uint32_t)tag >> 4;
-        if (tag & DT_FIRST) {
-            if (u == 0) {
-                double xy[20]; int type[10];
-                if ((tag & DT_HOST_DRAWS) && draws) {
-                    const double* dr = draws + (size_t)i * KUKA_DIST_DRAWS;
-                    for (int k = 0; k < 20; ++k) xy[k] = dr[18 + k];
-                    for (int k = 0; k < 10; ++k) type[k] = (int)dr[38 + k];
-                } else {
-                    // x = 0.5 + 0.15 U(-1, 1), y = 0 + 0.3 U(-1, 1) (kuka_rand_button_gym_env.py:63-64); the object type from the same stream
-                    for (int k = 0; k < 10; ++k) {
-                        const uint4 r = philox4x32_10(P.seed, genv, episode, PHILOX_PURPOSE_DIST_PLACE + k);
-                        xy[2 * k] = 0.5 + 0.15 * (-1.0 + 2.0 * philox_u01(r.x, r.y));
-                        xy[2 * k + 1] = 0.3 * (-1.0 + 2.0 * philox_u01(r.z, r.w));
-                    }
-                    for (int k = 0; k < 10; k += 4) {
-                        const uint4 r = philox4x32_10(P.seed, genv, episode, PHILOX_PURPOSE_DIST_TYPE + k / 4);
-                        const uint32_t w[4] = {r.x, r.y, r.z, r.w};
-                        for (int j = 0; j < 4 && k + j < 10; ++j) type[k + j] = (int)__umulhi(w[j], 3u);   // randint(3)
-                    }
-                }
-                dc_place(sh.B, xy, type, (double)r3.y, (double)r3.z);
-            }
-            touch.body = 0u; touch.arm = 0u; clear = 1u;
-            __syncwarp(gmask);
-            for (int s2 = 0; s2 < 500; ++s2) {    // p.stepSimulation() x 500 of reset() (:242-247), the arm on its settle trajectory
-                const float4 a0 = __ldg(g.settle + 4 * s2), a1 = __ldg(g.settle + 4 * s2 + 1), a2 = __ldg(g.settle + 4 * s2 + 2), a3 = __ldg(g.settle + 4 * s2 + 3);
-                const float q[KK_NB] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w, a2.x, a2.y, a2.z, a2.w};
-                const int na = arm_spheres(P, q, arm);
-                dist_scene(P, S, a3.x, r3.y, r3.z);
-                dist_micro_step(g.A, S, sh, u, gmask, arm, na, nullptr, rows, touch);
-            }
-        }
-        const float q[KK_NB] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w, r2.x, r2.y, r2.z, r2.w};
-        const int na = arm_spheres(P, q, arm);
-        dist_scene(P, S, r3.x, r3.y, r3.z);
-        float imp[3];
-        const bool kick = (tag & DT_KICK) != 0;
-        if (kick) {
-            // np.random.normal(size=(3,)), z dropped (:119-121): two normals of the env's stream
-            const uint4 r = philox4x32_10(P.seed, genv, episode, PHILOX_PURPOSE_DIST_KICK);
-            const double u1 = philox_u01(r.x, r.y), u2 = philox_u01(r.z, r.w);
-            const double rad = sqrt(-2.0 * log(1.0 - u1));
-            dc_kick(rad * cos(6.283185307179586 * u2), rad * sin(6.283185307179586 * u2), S.dt, imp);
-        }
-        dist_micro_step(g.A, S, sh, u, gmask, arm, na, kick ? imp : (const float*)nullptr, rows, touch);
-    }
-    for (int j = u; j < DC_NBODY * DC_B_WORDS; j += DIST_LANES) gb[j] = sh.B[j];
-    // the group's touch masks: OR over the lanes, on top of the stored ones unless a placement cleared them
-    for (int off = DIST_LANES / 2; off > 0; off >>= 1) {
-        touch.body |= __shfl_xor_sync(gmask, touch.body, off);
-        touch.arm |= __shfl_xor_sync(gmask, touch.arm, off);
-    }
-    if (u == 0) {
-        if (!clear) { touch.body |= g.touch[2 * i]; touch.arm |= g.touch[2 * i + 1]; }
-        g.touch[2 * i] = touch.body; g.touch[2 * i + 1] = touch.arm;
-    }
 }
 
 // ---- host side -------------------------------------------------------------------------------
@@ -897,81 +682,55 @@ void free_state(KukaState& a) {
 }
 
 #define KUKA_SMEM_BYTES ((size_t)(((KC_CONST_WORDS + 31) / 32) * 32 + 32 * KC_ES) * sizeof(float))   /* 4 warps x 8 env slots */
-template <bool J, bool T2, bool PF, bool CO>
+template <bool J, bool T2, bool PF, bool CO, bool TR>
 cudaError_t kuka_launch_inst(const KukaDev& d, const KukaNext& nx, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions,
                              const float* noise, const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret,
-                             int32_t* ep_len, float* snap) {
+                             int32_t* ep_len, float* snap, float4* trace, int* trace_len) {
     const size_t smem = CO ? KUKA_SMEM_BYTES : 0;
-    static bool attr_set = false;
-    if (CO && !attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kuka_kernel<J, T2, PF, CO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    kuka_kernel<J, T2, PF, CO><<<grid, block, smem, st>>>(d, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap, nx,
-                                                          nullptr, nullptr);
+    if constexpr (CO) { if (const cudaError_t e = srl_smem_opt_in<kuka_kernel<J, T2, PF, CO, TR>>(smem)) return e; }
+    kuka_kernel<J, T2, PF, CO, TR><<<grid, block, smem, st>>>(d, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap, nx,
+                                                              trace, trace_len);
     return cudaGetLastError();
 }
 
-// the traced instantiations (single button, no records): distractor bodies
-template <bool J, bool CO>
-cudaError_t kuka_launch_trace(const KukaDev& d, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions,
-                              const float* noise, const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret,
-                              int32_t* ep_len, float* snap, float4* trace, int* trace_len) {
-    const size_t smem = CO ? KUKA_SMEM_BYTES : 0;
-    static bool attr_set = false;
-    if (CO && !attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kuka_kernel<J, false, false, CO, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        attr_set = true;
-    }
-    kuka_kernel<J, false, false, CO, true><<<grid, block, smem, st>>>(d, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len,
-                                                                        snap, KukaNext{}, trace, trace_len);
-    return cudaGetLastError();
-}
-
-// One instantiation per (action_joints, two_buttons, four lanes per env): the default kernel pays nothing for the variants.  With
-// next-episode records (`nx`, single-button kinds with IK actions only) the PREFETCH instantiation of the same layout.
+// One instantiation per (action_joints, two_buttons, four lanes per env) at inst[action_joints | two_buttons << 1 | coop << 2]: the default
+// kernel pays nothing for the variants.  With a trace (distractor bodies: single button, no records; `trace_len` null for the settle) the
+// TRACE one at inst[8 + (action_joints | coop << 1)]; with next-episode records (`nx`, single-button IK kinds) PREFETCH at inst[12 + coop].
 cudaError_t kuka_launch(const KukaDev& d, const KukaNext* nx, int grid, int block, cudaStream_t st, int n, int op, int T, const void* actions,
                         const float* noise, const uint8_t* mask, const double* draws, float* obs, float* rew, uint8_t* done, float* ep_ret,
-                        int32_t* ep_len, float* snap) {
-    using Launch = decltype(&kuka_launch_inst<false, false, false, false>);
-    static const Launch plain[8] = {kuka_launch_inst<false, false, false, false>, kuka_launch_inst<true, false, false, false>,
-                                    kuka_launch_inst<false, true, false, false>,  kuka_launch_inst<true, true, false, false>,
-                                    kuka_launch_inst<false, false, false, true>,  kuka_launch_inst<true, false, false, true>,
-                                    kuka_launch_inst<false, true, false, true>,   kuka_launch_inst<true, true, false, true>};
-    const Launch launch = nx ? (d.coop ? kuka_launch_inst<false, false, true, true> : kuka_launch_inst<false, false, true, false>)
-                             : plain[(d.P.action_joints ? 1 : 0) | (d.P.two_buttons ? 2 : 0) | (d.coop ? 4 : 0)];
-    return launch(d, nx ? *nx : KukaNext{}, grid, block, st, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap);
+                        int32_t* ep_len, float* snap, float4* trace = nullptr, int* trace_len = nullptr) {
+    using Launch = decltype(&kuka_launch_inst<false, false, false, false, false>);
+    static const Launch inst[14] = {kuka_launch_inst<false, false, false, false, false>, kuka_launch_inst<true, false, false, false, false>,
+                                    kuka_launch_inst<false, true, false, false, false>,  kuka_launch_inst<true, true, false, false, false>,
+                                    kuka_launch_inst<false, false, false, true, false>,  kuka_launch_inst<true, false, false, true, false>,
+                                    kuka_launch_inst<false, true, false, true, false>,   kuka_launch_inst<true, true, false, true, false>,
+                                    kuka_launch_inst<false, false, false, false, true>,  kuka_launch_inst<true, false, false, false, true>,
+                                    kuka_launch_inst<false, false, false, true, true>,   kuka_launch_inst<true, false, false, true, true>,
+                                    kuka_launch_inst<false, false, true, false, false>,  kuka_launch_inst<false, false, true, true, false>};
+    const int j = d.P.action_joints ? 1 : 0, co = d.coop ? 1 : 0;
+    const Launch launch = nx ? inst[12 + co] : trace ? inst[8 + (j | co << 1)] : inst[j | (d.P.two_buttons ? 2 : 0) | co << 2];
+    return launch(d, nx ? *nx : KukaNext{}, grid, block, st, n, op, T, actions, noise, mask, draws, obs, rew, done, ep_ret, ep_len, snap,
+                  trace, trace_len);
 }
 
-void grid_for(const srl_sim* s, const KukaDev* d, int& grid, int& block) {
-    const int warps = (s->n + d->epw - 1) / d->epw;
+void grid_for(const srl_sim* s, int& grid, int& block) {
+    const int warps = (s->n + s->kuka->epw - 1) / s->kuka->epw;
     block = 128;
     grid = (warps * 32 + block - 1) / block;
 }
 
-// a traced kuka_kernel launch of at most `steps` micro-steps per env, then distractor_kernel over the same micro-steps
-int dist_launch(srl_sim* s, int op, int T, size_t steps, const void* actions, const float* noise, const uint8_t* mask, const double* draws,
-                float* obs, float* rew, uint8_t* done, float* ep_ret, int32_t* ep_len, cudaStream_t st) {
-    KukaDev* d = s->kuka;
-    DistDev* g = s->dist;
-    const size_t N = (size_t)s->n;
-    if (steps > g->cap) {
-        SRL_CUDA_OK(cudaStreamSynchronize(st));
-        if (g->trace) cudaFree(g->trace);
-        g->trace = nullptr; g->cap = 0;
-        SRL_CUDA_OK(cudaMalloc(&g->trace, steps * 4 * N * sizeof(float4)));
-        g->cap = steps;
-    }
-    SRL_CUDA_OK(cudaMemsetAsync(g->trace_len, 0, N * sizeof(int), st));
-    int grid, block; grid_for(s, d, grid, block);
-    using Launch = decltype(&kuka_launch_trace<false, false>);
-    static const Launch inst[4] = {kuka_launch_trace<false, false>, kuka_launch_trace<true, false>, kuka_launch_trace<false, true>, kuka_launch_trace<true, true>};
-    SRL_CUDA_OK(inst[(d->P.action_joints ? 1 : 0) | (d->coop ? 2 : 0)](*d, grid, block, st, s->n, op, T, actions, noise, mask, draws, obs, rew, done,
-                                                                       ep_ret, ep_len, nullptr, g->trace, g->trace_len));
-    distractor_kernel<<<(s->n + DIST_ENVS_PER_BLOCK - 1) / DIST_ENVS_PER_BLOCK, DIST_BLOCK, 0, st>>>(*d, *g, s->n, draws);
-    SRL_CUDA_OK(cudaGetLastError());
+// The 500 zero-action settle steps of reset() for one env, from resetJointState at the initial joint vector: h[0..28] = the reset
+// snapshot (q, qd, commanded end effector, glider q, qd).  With `trace`, the traced instantiation also records the arm's trajectory.
+int settle(srl_sim* s, float4* trace, float* h) {
+    KukaDev one = *s->kuka;
+    one.epw = 1;
+    for (int k = 0; k < KK_NB; ++k) one.P.snap_q[k] = s->kuka_q0[k];
+    float* snap = nullptr;
+    SRL_CUDA_OK(cudaMalloc(&snap, 32 * sizeof(float)));
+    SRL_CUDA_OK(kuka_launch(one, nullptr, 1, 32, 0, 1, KUKA_OP_SETTLE, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, snap, trace, nullptr));
+    SRL_CUDA_OK(cudaMemcpy(h, snap, 29 * sizeof(float), cudaMemcpyDeviceToHost));
+    cudaFree(snap);
     return 0;
 }
 
@@ -1001,15 +760,8 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
     d->coop = epw <= 8 ? 1 : 0;
     // the 500 settle steps of reset(), once
     for (int k = 0; k < KK_NB; ++k) s->kuka_q0[k] = d->P.snap_q[k];
-    float* snap = nullptr;
-    SRL_CUDA_OK(cudaMalloc(&snap, 32 * sizeof(float)));
-    { const int save_epw = d->epw; d->epw = 1;
-      SRL_CUDA_OK(kuka_launch(*d, nullptr, 1, 32, 0, 1, KUKA_OP_SETTLE, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, snap));
-      d->epw = save_epw; }
-    SRL_CUDA_OK(cudaGetLastError());
-    float h[32];
-    SRL_CUDA_OK(cudaMemcpy(h, snap, sizeof(h), cudaMemcpyDeviceToHost));
-    cudaFree(snap);
+    float h[29];
+    if (settle(s, nullptr, h)) return 1;
     for (int i = 0; i < KK_NB; ++i) { d->P.snap_q[i] = h[i]; d->P.snap_qd[i] = h[KK_NB + i]; }
     d->P.snap_ee[0] = h[24]; d->P.snap_ee[1] = h[25]; d->P.snap_ee[2] = h[26]; d->P.snap_qb = h[27]; d->P.snap_qdb = h[28];
     s->launches += 1;
@@ -1031,11 +783,7 @@ int kuka_alloc(srl_sim* s, const void* blob, size_t bytes) {
 void kuka_free(srl_sim* s) {
     KukaDev* d = s->kuka;
     if (!d) return;
-    if (DistDev* g = s->dist) {
-        cudaFree(g->body); cudaFree(g->touch); cudaFree(g->trace); cudaFree(g->trace_len); cudaFree(g->settle);
-        delete g;
-        s->dist = nullptr;
-    }
+    dist_free(s);
     free_state(*d);
     delete d;
     s->kuka = nullptr;
@@ -1050,48 +798,46 @@ void kuka_free(srl_sim* s) {
 }
 
 int kuka_launch_reset(srl_sim* s, const uint8_t* mask, const double* draws, float* obs, cudaStream_t st) {
-    KukaDev* d = s->kuka;
     s->kuka_started = true;
-    if (s->dist) return dist_launch(s, KUKA_OP_RESET, 0, N_RANDOM_ACTIONS_AT_INIT, nullptr, nullptr, mask, draws, obs, nullptr, nullptr, nullptr, nullptr, st);
-    int grid, block; grid_for(s, d, grid, block);
-    SRL_CUDA_OK(kuka_launch(*d, nullptr, grid, block, st, s->n, KUKA_OP_RESET, 0, nullptr, nullptr, mask, draws, obs, nullptr, nullptr, nullptr, nullptr, nullptr));
-    SRL_CUDA_OK(cudaGetLastError());
-    return 0;
+    float4* trace = nullptr; int* trace_len = nullptr;
+    if (s->dist && dist_trace(s, N_RANDOM_ACTIONS_AT_INIT, st, &trace, &trace_len)) return 1;
+    int grid, block; grid_for(s, grid, block);
+    SRL_CUDA_OK(kuka_launch(*s->kuka, nullptr, grid, block, st, s->n, KUKA_OP_RESET, 0, nullptr, nullptr, mask, draws, obs, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, trace, trace_len));
+    return s->dist ? dist_advance(s, draws, st) : 0;
 }
 
 int kuka_launch_rollout(srl_sim* s, int T, const void* actions, const float* noise, float* obs, float* rew, uint8_t* done,
                         float* ep_ret, int32_t* ep_len, cudaStream_t st) {
-    KukaDev* d = s->kuka;
     s->kuka_started = true;
-    if (s->dist)   // an env step is at most action_repeat micro-steps, a reset() inside the launch 5 more
-        return dist_launch(s, KUKA_OP_ROLLOUT, T, (size_t)T * (size_t)(s->cfg.action_repeat + N_RANDOM_ACTIONS_AT_INIT), actions, noise, nullptr,
-                           nullptr, obs, rew, done, ep_ret, ep_len, st);
-    int grid, block; grid_for(s, d, grid, block);
+    float4* trace = nullptr; int* trace_len = nullptr;
+    // an env step is at most action_repeat micro-steps, a reset() inside the launch 5 more
+    if (s->dist && dist_trace(s, (size_t)T * (size_t)(s->cfg.action_repeat + N_RANDOM_ACTIONS_AT_INIT), st, &trace, &trace_len)) return 1;
+    int grid, block; grid_for(s, grid, block);
+    KukaNext nx{};
+    bool capturing = false;
     if (s->kuka_next) {         // the rollout path that takes a ready next-episode record instead of resetting inside the launch
         cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
         cudaStreamIsCapturing(st, &cap);
-        const bool capturing = cap != cudaStreamCaptureStatusNone;   // events recorded outside a capture cannot be waited for inside it
+        capturing = cap != cudaStreamCaptureStatusNone;   // events recorded outside a capture cannot be waited for inside it
         if (s->pf_pending && !capturing) { SRL_CUDA_OK(cudaStreamWaitEvent(st, s->pf_ev, 0)); s->pf_pending = false; }
-        KukaNext nx = *s->kuka_next;
+        nx = *s->kuka_next;
         nx.helper = 1;          // the first idle slot of every warp advances one incomplete record of its warp's envs by up to T micro-steps
-        SRL_CUDA_OK(kuka_launch(*d, &nx, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr));
-        if (!capturing) { SRL_CUDA_OK(cudaEventRecord(s->roll_ev, st)); s->roll_ev_valid = true; }
     }
-    else
-        SRL_CUDA_OK(kuka_launch(*d, nullptr, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done, ep_ret, ep_len, nullptr));
-    SRL_CUDA_OK(cudaGetLastError());
-    return 0;
+    SRL_CUDA_OK(kuka_launch(*s->kuka, s->kuka_next ? &nx : nullptr, grid, block, st, s->n, KUKA_OP_ROLLOUT, T, actions, noise, nullptr, nullptr, obs, rew, done,
+                            ep_ret, ep_len, nullptr, trace, trace_len));
+    if (s->kuka_next && !capturing) { SRL_CUDA_OK(cudaEventRecord(s->roll_ev, st)); s->roll_ev_valid = true; }
+    return s->dist ? dist_advance(s, nullptr, st) : 0;
 }
 
 // Refresh the next-episode records of the envs that consumed theirs (or never had one).  Asynchronous on `st`; meant for a side stream, it may
 // run concurrently with step / rollout launches of the same handle (flag + fence hand-over, see KukaNext).  A no-op when the feature is off.
 int kuka_launch_prefetch(srl_sim* s, cudaStream_t st) {
-    KukaDev* d = s->kuka;
     if (!s->kuka_next) return 0;
-    int grid, block; grid_for(s, d, grid, block);
+    int grid, block; grid_for(s, grid, block);
     // never concurrent with a rollout launch of the handle: its idle slots advance the same records
     if (s->roll_ev_valid) SRL_CUDA_OK(cudaStreamWaitEvent(st, s->roll_ev, 0));
-    SRL_CUDA_OK(kuka_launch(*d, s->kuka_next, grid, block, st, s->n, KUKA_OP_PREFETCH, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
+    SRL_CUDA_OK(kuka_launch(*s->kuka, s->kuka_next, grid, block, st, s->n, KUKA_OP_PREFETCH, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr));
     SRL_CUDA_OK(cudaEventRecord(s->pf_ev, st));
     s->pf_pending = true;
     s->launches += 1;
@@ -1099,40 +845,13 @@ int kuka_launch_prefetch(srl_sim* s, cudaStream_t st) {
 }
 
 int kuka_set_distractors(srl_sim* s, const void* blob, size_t bytes) {
-    if (s->kind != SRL_ENV_KUKA_RAND_BUTTON) { srl_set_error("set_distractors: only KukaRandButtonGymEnv-v0 has distractor bodies"); return 1; }
-    if (s->kuka_started) { srl_set_error("set_distractors: must be called between srl_sim_create and the first reset"); return 1; }
-    if (s->kuka_next) { srl_set_error("set_distractors: not available together with srl_cfg.prefetch_resets"); return 1; }
-    if (s->dist) { srl_set_error("set_distractors: already set"); return 1; }
-    if (!blob) { srl_set_error("set_distractors: null asset blob"); return 1; }
-    if (const char* err = dc_blob_error((const double*)blob, bytes)) { srl_set_error("set_distractors: %s", err); return 1; }
-    KukaDev* d = s->kuka;
-    DistDev* g = new DistDev();
-    memset(g, 0, sizeof(*g));
-    s->dist = g;   // freed by kuka_free, also when this call fails below
-    dc_assets_from_blob((const double*)blob, g->A);
-    const size_t N = (size_t)s->n;
-    SRL_CUDA_OK(cudaMalloc(&g->body, N * DC_NBODY * DC_B_WORDS * sizeof(float)));
-    SRL_CUDA_OK(cudaMemset(g->body, 0, N * DC_NBODY * DC_B_WORDS * sizeof(float)));
-    SRL_CUDA_OK(cudaMalloc(&g->touch, N * 2 * sizeof(uint32_t)));
-    SRL_CUDA_OK(cudaMemset(g->touch, 0, N * 2 * sizeof(uint32_t)));
-    SRL_CUDA_OK(cudaMalloc(&g->trace_len, N * sizeof(int)));
-    SRL_CUDA_OK(cudaMemset(g->trace_len, 0, N * sizeof(int)));
+    float4* trajectory = nullptr;
+    if (dist_alloc(s, blob, bytes, &trajectory)) return 1;
     // the arm's settle trajectory: the settle launch of kuka_alloc again, traced (the same instructions, so the same trajectory)
-    SRL_CUDA_OK(cudaMalloc(&g->settle, 500 * 4 * sizeof(float4)));
-    float* snap = nullptr;
-    SRL_CUDA_OK(cudaMalloc(&snap, 32 * sizeof(float)));
-    KukaDev one = *d;
-    one.epw = 1;
-    for (int k = 0; k < KK_NB; ++k) one.P.snap_q[k] = s->kuka_q0[k];   // the settle starts from resetJointState at the initial joint vector
-    using Launch = decltype(&kuka_launch_trace<false, false>);
-    const Launch inst[4] = {kuka_launch_trace<false, false>, kuka_launch_trace<true, false>, kuka_launch_trace<false, true>, kuka_launch_trace<true, true>};
-    SRL_CUDA_OK(inst[(d->P.action_joints ? 1 : 0) | (d->coop ? 2 : 0)](one, 1, 32, 0, 1, KUKA_OP_SETTLE, 0, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                                       nullptr, nullptr, nullptr, nullptr, snap, g->settle, nullptr));
-    SRL_CUDA_OK(cudaDeviceSynchronize());
+    float h[29];
+    if (settle(s, trajectory, h)) return 1;
     // the traced settle must be the trajectory kuka_alloc's settle produced: its end state is the reset snapshot, bit for bit
-    float h[32];
-    SRL_CUDA_OK(cudaMemcpy(h, snap, sizeof(h), cudaMemcpyDeviceToHost));
-    cudaFree(snap);
+    const KukaDev* d = s->kuka;
     bool same = memcmp(h + 27, &d->P.snap_qb, sizeof(float)) == 0 && memcmp(h + 28, &d->P.snap_qdb, sizeof(float)) == 0;
     for (int k = 0; k < KK_NB; ++k) same = same && memcmp(h + k, &d->P.snap_q[k], sizeof(float)) == 0 && memcmp(h + KK_NB + k, &d->P.snap_qd[k], sizeof(float)) == 0;
     if (!same) { srl_set_error("set_distractors: the traced settle does not reproduce the reset snapshot"); return 1; }
@@ -1235,27 +954,8 @@ int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
         return 0;
     }
 #endif
-    case SRL_F_DISTRACTORS: {
-        if (!need(DC_NBODY * 9, 8)) return 1;
-        for (size_t i = 0; i < N * DC_NBODY * 9; ++i) D[i] = 0.0;
-        if (const DistDev* g = s->dist) {
-            std::vector<float> h(N * DC_NBODY * DC_B_WORDS);
-            SRL_CUDA_OK(cudaMemcpy(h.data(), g->body, h.size() * sizeof(float), cudaMemcpyDeviceToHost));
-            for (size_t i = 0; i < N * DC_NBODY; ++i) {
-                const float* b = h.data() + i * DC_B_WORDS;
-                double* o = D + i * 9;
-                for (int a = 0; a < 7; ++a) o[a] = b[DC_B_P + a];   // position, quaternion (x y z w)
-                o[7] = b[DC_B_TYPE]; o[8] = b[DC_B_PRESENT];
-            }
-        }
-        return 0;
-    }
-    case SRL_F_DISTRACTOR_TOUCH: {
-        if (!need(2, 4)) return 1;
-        for (size_t i = 0; i < 2 * N; ++i) I[i] = 0;
-        if (const DistDev* g = s->dist) SRL_CUDA_OK(cudaMemcpy(I, g->touch, N * 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-        return 0;
-    }
+    case SRL_F_DISTRACTORS: case SRL_F_DISTRACTOR_TOUCH:
+        return dist_get_state(s, field, dst, bytes);
     case SRL_F_NEXT_RECORD: {
         if (!need(3, 4)) return 1;
         const KukaNext* nx = s->kuka_next;

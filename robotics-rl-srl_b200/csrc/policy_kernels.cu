@@ -350,14 +350,8 @@ int srl_policy_act(const srl_mlp_policy* p, int n, const float* obs, uint64_t* r
     }
     if (!p->pi_w1 || !p->pi_b1 || !p->pi_w2 || !p->pi_b2 || !p->pi_w3 || !p->pi_b3 || !p->vf_w1 || !p->vf_b1 || !p->vf_w2 || !p->vf_b2 ||
         !p->vf_w3 || !p->vf_b3 || (!p->discrete && !p->logstd)) { srl_set_error("policy_act: null weight pointer"); return 1; }
-    static bool attr_set[64] = {};     // > 48 KB of dynamic shared memory needs the opt-in once per device context
     constexpr size_t smem = policy_smem_bytes();
-    int dev = 0;
-    SRL_CUDA_OK(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        SRL_CUDA_OK(cudaFuncSetAttribute(policy_act_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
+    SRL_CUDA_OK(srl_smem_opt_in<policy_act_kernel>(smem));
     PolicyArgs a;
     a.p = *p; a.n = n; a.obs = obs; a.rng = reinterpret_cast<unsigned long long*>(rng); a.env_offset = env_offset;
     a.obs_buf = obs_buf; a.act_env = act_env; a.act_buf = act_buf; a.logp = logp; a.value = value;

@@ -530,14 +530,8 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
     if (ctas <= 0) { srl_set_error("ppo2_grad: no CUDA device"); return 1; }
     const Seg seg = make_seg(p->obs_dim, p->n_out, p->discrete);
     if (workspace_bytes < 2048 + sizeof(float) * (size_t)seg.P * (size_t)ctas) { srl_set_error("ppo2_grad: workspace too small (srl_ppo2_workspace_bytes)"); return 1; }
-    static bool attr_set[64] = {};
-    int dev = 0;
-    SRL_CUDA_OK(cudaGetDevice(&dev));
     constexpr size_t smem = grad_smem_bytes();
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        SRL_CUDA_OK(cudaFuncSetAttribute(ppo2_grad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
+    SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_kernel>(smem));
     cudaStream_t st = (cudaStream_t)stream;
     double* stats = reinterpret_cast<double*>(workspace);
     float* partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 2048);

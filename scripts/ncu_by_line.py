@@ -43,7 +43,7 @@ for f, (s_, i_) in sorted(files.items(), key=lambda x: -x[1][0]):
 # function ranges
 import os
 root = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "robotics-rl-srl_b200", "csrc")
-for fname in ("kuka_coop.cuh", "kuka_device.cuh", "kuka_kernels.cu"):
+for fname in ("kuka_coop.cuh", "kuka_device.cuh", "kuka_kernels.cu", "distractor_kernels.cu"):
     try:
         src = open(os.path.join(root, fname)).read().split("\n")
     except Exception:

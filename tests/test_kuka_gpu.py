@@ -244,6 +244,20 @@ def test_in_kernel_streams_and_sharding_invariance(cuda_backend, oracle_backend)
     assert np.abs(whole["target"] - o["target"]).max() < 1e-6
 
 
+def test_handle_on_every_device(cuda_lib):
+    """One process, one Kuka handle per visible device: the four-lane kernel's shared-memory opt-in belongs to a device context, so every
+    device must get it, and every device computes the same rollout bit for bit."""
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two visible devices")
+    from srl_sim.backend import Backend
+    runs = [_run(Backend(cuda_lib, dev), "KukaButtonGymEnv-v0", 40, 30, None, None, seed=3, max_steps=20)
+            for dev in range(torch.cuda.device_count())]
+    for r in runs[1:]:
+        for k in ("obs0", "obs", "rew", "done", "ep_len", "q", "qd", "counters"):
+            assert np.array_equal(runs[0][k], r[k]), k
+
+
 def test_full_size_properties_4096_envs(cuda_backend):
     """BASELINE config 2 size: 4096 envs, fused rollouts; size-independent invariants of the env."""
     n, T = 4096, 384
