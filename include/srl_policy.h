@@ -83,8 +83,10 @@ int srl_ppo2_grad(const srl_mlp_policy* policy, const srl_mlp_grads* grads, int 
 
 /* GAE(lambda) over one rollout (the backward recursion of stable-baselines' PPO2 runner): rew, value, done (1.0 where the episode ended at that
  * step), adv_out, ret_out are f32[n_steps, n_envs]; last_value f32[n_envs] is the value of the observation after the last step.
- *   delta_t = rew_t + gamma * V_{t+1} * (1 - done_t) - V_t;  adv_t = delta_t + gamma * lam * (1 - done_t) * adv_{t+1};  ret_t = adv_t + V_t */
-int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, float gamma, float lam,
+ *   delta_t = rew_t + gamma * V_{t+1} * (1 - done_t) - V_t;  adv_t = delta_t + gamma * lam * (1 - done_t) * adv_{t+1};  ret_t = adv_t + V_t
+ * gamma and lam are doubles: the float32 recursion uses fl32(gamma) and fl32(gamma * lam), the coefficients a float32 array expression with
+ * Python-float hyper-parameters uses (fl32(gamma) * fl32(lam) is another float for e.g. gamma = lam = 0.9). */
+int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, double gamma, double lam,
                  float* adv_out, float* ret_out, void* stream);
 
 #ifdef __cplusplus

@@ -549,11 +549,12 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
     return 0;
 }
 
-int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, float gamma, float lam,
+int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, double gamma, double lam,
                  float* adv_out, float* ret_out, void* stream) {
     if (!rew || !value || !done || !last_value || !adv_out || !ret_out) { srl_set_error("ppo2_gae: null argument"); return 1; }
     if (n_steps < 1 || n_envs < 1) { srl_set_error("ppo2_gae: bad shape"); return 1; }
-    gae_kernel<<<(n_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n_steps, n_envs, rew, value, done, last_value, gamma, (float)((double)gamma * (double)lam), adv_out, ret_out);
+    // the coefficients of the torch recursion: `gamma * nextval` rounds gamma to float32, `gamma * lam * nonterminal` rounds the double product
+    gae_kernel<<<(n_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n_steps, n_envs, rew, value, done, last_value, (float)gamma, (float)(gamma * lam), adv_out, ret_out);
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }

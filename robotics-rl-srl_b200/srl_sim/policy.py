@@ -9,7 +9,7 @@ Reference pieces replaced: stable-baselines' ``PPO2`` runner ``model.step(obs)``
 There is no CPU fallback here either: :class:`FusedPolicy` needs the CUDA library and CUDA tensors.
 """
 import ctypes
-from ctypes import POINTER, Structure, byref, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64, c_void_p
+from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64, c_void_p
 
 HIDDEN, MAX_OBS, MAX_OUT = 64, 8, 8
 POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae"]
@@ -41,7 +41,7 @@ def bind(cdll):
     cdll.srl_ppo2_grad.argtypes = [POINTER(SrlMlpPolicy), POINTER(SrlMlpGrads), c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                    c_float, c_float, c_float, c_void_p, c_size_t, c_void_p]
     cdll.srl_ppo2_gae.restype = c_int
-    cdll.srl_ppo2_gae.argtypes = [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p, c_void_p]
+    cdll.srl_ppo2_gae.argtypes = [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_void_p, c_void_p, c_void_p]
     return cdll
 
 
