@@ -65,7 +65,7 @@ enum {
 #define KC_OFF_BIAS (KC_OFF_MA + KK_NB * KC_MS)    // [12] bias torques
 #define KC_OFF_ROWS (((KC_OFF_BIAS + KK_NB + 3) / 4) * 4)   // 3 * KK_MAXC constraint rows of KC_RS words in the KK_ROW_* layout (kuka_params.cuh), 16-byte aligned
 #define KC_RS 36                                   // = 4 (mod 32): the 4 lanes that fill 4 consecutive rows hit different banks; a multiple of 4 words
-#define KC_OFF_WT (KC_OFF_ROWS + 3 * KK_MAXC * KC_RS)   // watch matrix [12][4]: Wt[i][c] = W'_i of normal row c (0 for c >= nc) -- one 128-bit load per motor row
+#define KC_OFF_WT (KC_OFF_ROWS + 3 * KK_MAXC * KC_RS)   // watch matrix [12][4]: Wt[i][c] = W'_i of normal row c < nc, written and read by lane c of the group
 #define KC_OFF_END (KC_OFF_WT + KK_NB * 4)
 #define KC_OFF_CAND KC_OFF_MA                      // collision candidates per sphere (count, then KC_CANDS records of 8 words: shape, dist, n, pt):
 #define KC_CANDS 3                                 // consumed by the collect phase before the dynamics write M, L, rows -- same storage
@@ -502,10 +502,6 @@ KC_F void kc_ph_rows(const S& s, const KukaParams& P, const float (&A)[KK_NB][KK
         s[ro + KK_ROW_INVD] = 1.0f / D;
         const float pen = s[co + 2];
         s[ro + KK_ROW_TGT] = (r < nc ? (pen > 0.f ? -pen * P.inv_dt : -P.erp * pen * P.inv_dt) : 0.f) - off;
-    }
-    if (SCALED && u >= nc) {             // watch matrix columns without a contact: zeros (lane u owns column u; columns < nc were written with row u above)
-#pragma unroll
-        for (int i = 0; i < KK_NB; ++i) s[KC_OFF_WT + 4 * i + u] = 0.f;
     }
 }
 

@@ -38,9 +38,11 @@
 // Diagnostic build (scripts/build_variant.sh phases -DKK_PHASES, scripts/kuka_phase_timing.py): clock64() accumulators per phase of the
 // micro-step loop, in registers, stored per env slot at the end of the launch.  Separate from KK_TIMING, whose convergence probe adds
 // instructions to every sweep row.  KK_PH(clk, k) charges the cycles since the previous mark to phase k; without KK_PHASES it is empty.
-enum { KK_PH_KIN = 0, KK_PH_IK, KK_PH_DYN, KK_PH_CHOL, KK_PH_SETUP, KK_PH_FAST, KK_PH_GENERAL, KK_PH_ENV, KK_NPH };
+// The fast sweeps are charged to one of two phases, by the copy of the loop the warp ran (no lane watching a contact, or the watch copy);
+// `nwatch` counts the physics steps of the slot that ran the watch copy.
+enum { KK_PH_KIN = 0, KK_PH_IK, KK_PH_DYN, KK_PH_CHOL, KK_PH_SETUP, KK_PH_FAST_QUIET, KK_PH_FAST_WATCH, KK_PH_GENERAL, KK_PH_ENV, KK_NPH };
 #if defined(KK_PHASES) && defined(__CUDACC__)
-struct KkPhaseClock { long long last; long long acc[KK_NPH]; };
+struct KkPhaseClock { long long last; long long acc[KK_NPH]; unsigned nwatch; };
 #define KK_PH(clk, k) do { if (clk) { const long long t_ = clock64(); (clk)->acc[k] += t_ - (clk)->last; (clk)->last = t_; } } while (0)
 #else
 struct KkPhaseClock { long long dummy; };
@@ -738,27 +740,27 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         _Pragma("unroll")                                                                                              \
         for (int j = 0; j < KK_NB; ++j) v[j] = fmaf(KK_A(j, i), d, v[j]);                                              \
     }
-    // the same with the contact watch folded in: J'_c . v' of the (up to 4) watched normal rows is carried incrementally -- a motor row's step d
-    // moves it by W'_ci d (W' = A' J'^T: the column the general loop would apply) -- as 4 independent FFMA per row off the loop-carried path,
-    // fed by one 128-bit load of the watch matrix; recomputing the 14-term dot per contact after every sweep cost on the order of 100 cycles per
-    // contact and sweep on the single resident warp, and a step's time grew with each contact
+    // the same with the contact watch folded in: J'_u . v' of the watched normal row u of this lane is carried incrementally -- a motor row's
+    // step d moves it by W'_ui d (W' = A' J'^T: the column the general loop would apply) -- as one FFMA per row off the loop-carried path;
+    // recomputing the 14-term dot per contact after every sweep cost on the order of 100 cycles per contact and sweep on the single resident
+    // warp, and a step's time grew with each contact
 #define KK_MOTOR_ROWS_WATCH()                                                                                          \
     _Pragma("unroll")                                                                                                  \
     for (int i = 0; i < KK_NB; ++i) {                                                                                  \
-        const kk_f4 w4 = *reinterpret_cast<const kk_f4*>(wt + 4 * i);                                                  \
         const float s = __saturatef(fmaf(-cs[i], v[i], lam[i]));                                                       \
         const float d = s - lam[i];                                                                                    \
         lam[i] += d;                                                                                                   \
         KK_PROBE_D(d)                                                                                                  \
         _Pragma("unroll")                                                                                              \
         for (int j = 0; j < KK_NB; ++j) v[j] = fmaf(KK_A(j, i), d, v[j]);                                              \
-        wjv[0] = fmaf(w4.x, d, wjv[0]); wjv[1] = fmaf(w4.y, d, wjv[1]); wjv[2] = fmaf(w4.z, d, wjv[2]); wjv[3] = fmaf(w4.w, d, wjv[3]); \
+        wjv = fmaf(wl[i], d, wjv);                                                                                     \
     }
     int it0 = 0;                 // first sweep the general loop still has to do
 #if defined(KK_TIMING)
     bool kk_probe_any = false; int kk_probe_sweep = 0, kk_probe_conv = 0;
 #endif
     bool resume_mid_sweep = false;  // the fast loop already ran the motor + button rows of sweep it0
+    bool watching = false;          // the warp ran the watch copy of the fast loop (phase attribution only)
     KK_PH(ph, KK_PH_SETUP);
     if ((lim_lo_mask | lim_hi_mask) == 0u) {
         // FAST LOOP (no arm joint on a limit): straight-line sweep, registers only.  Contact rows of the manifold are
@@ -772,6 +774,10 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         asm volatile("mov.f32 %0, %1;" : "=f"(hi_hi) : "f"(bl_hi_hi));
         asm volatile("mov.f32 %0, %1;" : "=f"(lo_t) : "f"(bl_lo_t));
         asm volatile("mov.f32 %0, %1;" : "=f"(hi_t) : "f"(bl_hi_t));
+        asm volatile("mov.f32 %0, %0;" : "+f"(b_hi));   // else an indexed constant load (btn_maximp or btn_idle_imp) in every sweep
+        // and the motor rows' 1 / (sigma_i^2 A_ii): left transparent, ptxas recomputes them in every sweep (12 FMUL + constant loads)
+#pragma unroll
+        for (int i = 0; i < KK_NB; ++i) asm volatile("mov.f32 %0, %0;" : "+f"(cs[i]));
         bool act = false;        // a watched contact row would activate in sweep `it - 1`
         bool more = true;
         int it = 0;
@@ -796,6 +802,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
 #else
             const bool quiet = false;
 #endif
+            watching = !quiet;
             // one sweep per loop iteration: two let ptxas rotate the lam registers instead of copying them, but double the loop body beyond
             // the ~6 KB L0 instruction cache (measured slower)
             if (quiet) {
@@ -826,30 +833,27 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
                     }
                 } while (more);
             } else {
-                // four lanes per env (<= 8 envs per warp): watched normal rows c < nc (slots c >= nc: zero column, threshold -inf -- they never
-                // fire): arm part of J' . v' carried in wjv, the button DoF added when the row is tested
-                const float* wt = &sc[KC_OFF_WT];
-                float wjv[4], wthr[4], wjb[4], wjb2[4];
+                // four lanes per env (<= 8 envs per warp): the watch is dealt to the lanes -- lane u watches normal row u (u >= nc: zero
+                // column, threshold -1e30, it never fires) and carries its column of the watch matrix, the arm part of J'_u . v' (wjv) and
+                // the button coefficients, which enter when the row is tested.  One ballot, masked to the group's lanes, keeps `act` the same
+                // on all four: what follows the loop runs redundantly on every lane.  It votes over the active lanes (groups that left the loop
+                // are absent; a group's lanes never diverge inside it): with the group's own mask every group passes a different one, the warp
+                // splits at the WARPSYNC and the 8 groups vote one after the other in every sweep (that build's rollout measured 17 % slower
+                // than before the watch was dealt).
+                float wl[KK_NB], wjv = 0.f, wthr = -1e30f, wjb = 0.f, wjb2 = 0.f;
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    wjv[c] = 0.f; wthr[c] = -1e30f; wjb[c] = 0.f; wjb2[c] = 0.f;
-                    if (c < nc) {
-                        const float* row = KK_ROW_PTR(c);
-                        float Jr[16];
-                        KK_ROW_LOAD4(Jr, row, KK_ROW_J)
-                        float p0 = Jr[0] * v[0], p1 = Jr[1] * v[1], p2 = Jr[2] * v[2], p3 = Jr[3] * v[3];
-                        p0 = fmaf(Jr[4], v[4], p0); p1 = fmaf(Jr[5], v[5], p1); p2 = fmaf(Jr[6], v[6], p2); p3 = fmaf(Jr[7], v[7], p3);
-                        p0 = fmaf(Jr[8], v[8], p0); p1 = fmaf(Jr[9], v[9], p1); p2 = fmaf(Jr[10], v[10], p2); p3 = fmaf(Jr[11], v[11], p3);
-                        wjv[c] = (p0 + p1) + (p2 + p3);
-                        wthr[c] = Jr[KK_ROW_TGT]; wjb[c] = Jr[KK_NB]; wjb2[c] = Jr[KK_NB + 1];
-                    }
-                }
-                if (nc == 0) {           // a quiet env in a warp that watches: its watch matrix was not written this step
+                for (int i = 0; i < KK_NB; ++i) wl[i] = 0.f;
+                if (u < nc) {            // row u and column u were written by this lane (kc_ph_rows)
+                    const float* row = KK_ROW_PTR(u);
+                    float Jr[16];
+                    KK_ROW_LOAD4(Jr, row, KK_ROW_J)
+                    float p0 = Jr[0] * v[0], p1 = Jr[1] * v[1], p2 = Jr[2] * v[2], p3 = Jr[3] * v[3];
+                    p0 = fmaf(Jr[4], v[4], p0); p1 = fmaf(Jr[5], v[5], p1); p2 = fmaf(Jr[6], v[6], p2); p3 = fmaf(Jr[7], v[7], p3);
+                    p0 = fmaf(Jr[8], v[8], p0); p1 = fmaf(Jr[9], v[9], p1); p2 = fmaf(Jr[10], v[10], p2); p3 = fmaf(Jr[11], v[11], p3);
+                    wjv = (p0 + p1) + (p2 + p3);
+                    wthr = Jr[KK_ROW_TGT]; wjb = Jr[KK_NB]; wjb2 = Jr[KK_NB + 1];
 #pragma unroll
-                    for (int i = 0; i < KK_NB; ++i) sc[KC_OFF_WT + 4 * i + u] = 0.f;
-#if defined(__CUDACC__)
-                    __syncwarp(gmask);
-#endif
+                    for (int i = 0; i < KK_NB; ++i) wl[i] = sc[KC_OFF_WT + 4 * i + u];
                 }
 #pragma unroll 1
                 do {
@@ -858,12 +862,13 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
                     KK_PROBE_SWEEP()
                     ++it;
                     more = --left > 0;
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        float jv = fmaf(wjb[c], v[KK_NB], wjv[c]);
-                        if (TWOB) jv = fmaf(wjb2[c], v[ND - 1], jv);
-                        act = act | (wthr[c] - jv > 0.f);
-                    }
+                    float jv = fmaf(wjb, v[KK_NB], wjv);
+                    if (TWOB) jv = fmaf(wjb2, v[ND - 1], jv);
+#if defined(__CUDA_ARCH__)
+                    act = (__ballot_sync(__activemask(), wthr - jv > 0.f) & gmask) != 0u;
+#else
+                    act = wthr - jv > 0.f;
+#endif
                     if (act) more = false;
                 } while (more);
             }
@@ -874,7 +879,10 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         if (dbg && nc > 0) *dbg |= 1u;
 #endif
     }
-    KK_PH(ph, KK_PH_FAST);
+#if defined(KK_PHASES) && defined(__CUDACC__)
+    if (ph && watching) ++ph->nwatch;
+#endif
+    KK_PH(ph, watching ? KK_PH_FAST_WATCH : KK_PH_FAST_QUIET);
 #ifdef KK_TIMING
     if (dbg) *dbg |= ((unsigned)kk_probe_conv & 255u) << 24;
     if (dbg) { *dbg |= ((unsigned)nc & 15u) << 2; if (lim_lo_mask | lim_hi_mask) *dbg |= 64u; if (it0 < P.iters) *dbg |= 2u | ((unsigned)(P.iters - it0) & 255u) << 8; }

@@ -204,8 +204,8 @@ __device__ unsigned long long kk_timing[1 << 16];
 #endif
 #ifdef KK_PHASES
 // diagnostic build (scripts/build_variant.sh phases -DKK_PHASES): per env slot of the LAST launch, cycles spent in each phase of the micro-step
-// loop (KK_PH_* of kuka_device.cuh), then the number of physics steps the slot ran
-__device__ unsigned long long kk_phase[1 << 13][KK_NPH + 1];
+// loop (KK_PH_* of kuka_device.cuh), then the number of physics steps the slot ran and how many of them ran the watch copy of the fast loop
+__device__ unsigned long long kk_phase[1 << 13][KK_NPH + 2];
 #endif
 // TRACE (KukaRandButton with distractor bodies only): every micro-step also writes the arm configuration it starts from and what kind
 // of micro-step it is to `trace` (layout: kuka_state.cuh), and each env its number of micro-steps to `trace_len`; distractor_kernel
@@ -230,6 +230,7 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
     kk_ph_clk.last = clock64();
 #pragma unroll
     for (int k2 = 0; k2 < KK_NPH; ++k2) kk_ph_clk.acc[k2] = 0;
+    kk_ph_clk.nwatch = 0u;
 #else
     KkPhaseClock* const ph = nullptr;
 #endif
@@ -342,6 +343,7 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
 #pragma unroll
             for (int k2 = 0; k2 < KK_NPH; ++k2) kp[k2] = (unsigned long long)kk_ph_clk.acc[k2];
             kp[KK_NPH] = kk_nphys;
+            kp[KK_NPH + 1] = kk_ph_clk.nwatch;
         }
 #endif
         if constexpr (PREFETCH) {
@@ -949,7 +951,7 @@ int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
     }
 #endif
 #ifdef KK_PHASES
-    case 98: {   // diagnostic build: the per-slot phase cycles of the last launch, [slot][KK_NPH + 1]
+    case 98: {   // diagnostic build: the per-slot phase cycles of the last launch, [slot][KK_NPH + 2]
         if (cudaMemcpyFromSymbol(dst, kk_phase, bytes < sizeof(kk_phase) ? bytes : sizeof(kk_phase)) != cudaSuccess) return 1;
         return 0;
     }

@@ -4,7 +4,8 @@ micro-step loop and stores them at the end of the launch.
 
 Workload = bench.py's headline: KukaButtonGymEnv-v0, 4096 envs, T = 128, bench seeds and inputs, 3 warm-up rollouts, then LAUNCHES measured
 rollouts.  Per phase it prints cycles per physics step (median and max over slots), the phase's share of the slowest slot of each launch
-(the slot that ends last bounds the launch), and the same for the whole slot.  The phase clocks add a few registers (more spills) and
+(the slot that ends last bounds the launch), and the same for the whole slot.  The fast sweeps are split by the copy of the loop the
+warp ran (quiet: no env of the warp watches a contact; watch), with the share of physics steps that ran the watch copy.  The phase clocks add a few registers (more spills) and
 one clock read per mark, so the build runs a little slower than the shipped one: the split is the point, not the total."""
 import argparse, os, subprocess, sys
 import numpy as np
@@ -16,8 +17,9 @@ from srl_sim.backend import Backend
 from srl_sim.model import load_kuka_scene
 
 PHASES = ["kinematics + collision", "IK (float64 7x7)", "dynamics (CRBA + RNEA)", "Cholesky + M^-1", "v0 + row set-up + scaling + Euler",
-          "fast sweeps", "general loop", "env logic / loads / stores"]
+          "fast sweeps, quiet copy", "fast sweeps, watch copy", "general loop", "env logic / loads / stores"]
 NPH = len(PHASES)
+FAST_QUIET, FAST_WATCH = 5, 6
 
 
 def main():
@@ -46,9 +48,11 @@ def main():
     for _ in range(3):
         sim.rollout(T, acts, noise, obs, rew, done, ep_ret, ep_len, stream=st)
     torch.cuda.synchronize()
-    words = np.zeros((1 << 13, NPH + 1), np.uint64)
+    words = np.zeros((1 << 13, NPH + 2), np.uint64)
     per_step = []          # [launch] -> (live slots, NPH) cycles per physics step
     slowest = []           # [launch] -> (NPH,) cycles of the slowest slot
+    watch_share = []       # [launch] -> (live slots,) share of the slot's physics steps that ran the watch copy of the fast loop
+    slowest_watch = []     # [launch] -> that share for the slowest slot
     ms = []
     for _ in range(args.launches):
         words[:] = 0
@@ -59,9 +63,12 @@ def main():
         assert rc == 0, "srl_sim_get_state(98) failed: not a -DKK_PHASES build?"
         w = words.astype(np.float64)
         live = w[:, NPH] > 0
-        cyc, nphys = w[live, :NPH], w[live, NPH]
+        cyc, nphys, nwatch = w[live, :NPH], w[live, NPH], w[live, NPH + 1]
         per_step.append(cyc / nphys[:, None])
-        slowest.append(cyc[np.argmax(cyc.sum(axis=1))])
+        k_slow = np.argmax(cyc.sum(axis=1))
+        slowest.append(cyc[k_slow])
+        watch_share.append(nwatch / nphys)
+        slowest_watch.append(nwatch[k_slow] / nphys[k_slow])
     ps = np.concatenate(per_step)
     sl = np.mean(slowest, axis=0)
     print("KukaButtonGymEnv-v0, %d envs x T = %d, %d live slots, %d launches after 3 warm-ups: %s ms per launch (phase-clock build)"
@@ -72,6 +79,15 @@ def main():
     tot = ps.sum(axis=1)
     print("%-36s %14.0f %14.0f %15.1f%%" % ("total", np.median(tot), np.max(tot), 100.0))
     print("slowest slot: %.0f cycles per launch = %.3f ms at 1.98 GHz" % (sl.sum(), sl.sum() / 1.98e6))
+    ws = np.concatenate(watch_share)
+    print("physics steps that ran the watch copy: slowest slot %.1f%% (mean over launches), median slot %.1f%%, all slots %.1f%%"
+          % (100.0 * np.mean(slowest_watch), 100.0 * np.median(ws), 100.0 * np.mean(ws)))
+    # fast-sweep cycles per physics step of each copy, over the steps that ran it (the table above averages over all steps)
+    for name, k, share in (("quiet", FAST_QUIET, 1.0 - ws), ("watch", FAST_WATCH, ws)):
+        per = ps[:, k] / np.maximum(share, 1e-12)
+        per = per[share > 0]
+        if per.size:
+            print("fast sweeps, %s copy: median %.0f cycles per physics step that ran it (%d slots)" % (name, np.median(per), per.size))
 
 
 if __name__ == "__main__":
