@@ -44,6 +44,7 @@ struct MobileDev {
 struct KukaDev;   // kuka_state.cuh
 struct KukaNext;  // kuka_kernels.cu
 struct DistDev;   // distractor_kernels.cu
+struct SrlBodyLooks;  // render_core.h
 
 #define SRL_HOST_MAX_CHUNKS 16
 
@@ -117,3 +118,4 @@ int dist_trace(srl_sim* s, size_t steps, cudaStream_t st, float4** trace, int** 
 int dist_advance(srl_sim* s, const double* draws, cudaStream_t st);   // distractor_kernel through the micro-steps of the last traced launch
 void dist_free(srl_sim* s);
 int dist_get_state(srl_sim* s, int field, void* dst, size_t bytes);   // SRL_F_DISTRACTORS, SRL_F_DISTRACTOR_TOUCH
+const float* dist_render_bodies(const srl_sim* s, SrlBodyLooks* looks);   // [N][DC_NBODY][DC_B_WORDS] body poses + drawing table; nullptr: no bodies

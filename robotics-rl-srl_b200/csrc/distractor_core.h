@@ -83,6 +83,12 @@ DC_HD const char* dc_blob_error(const double* b, size_t bytes) {
             return "distractor asset blob: mass and inertia must be positive";
         if (!(w[DC_A_NSPH] >= 1.0 && w[DC_A_NSPH] <= DC_MAXSPH)) return "distractor asset blob: 1 to 4 collision spheres per body";
         if (!(w[DC_A_MU] >= 0.0)) return "distractor asset blob: negative friction";
+        // the drawing words (render_core.h: srl_distractor_prims)
+        if (!(w[DC_A_SHAPE] == 0.0 || w[DC_A_SHAPE] == 1.0)) return "distractor asset blob: DC_A_SHAPE must be 0 (box) or 1 (sphere)";
+        for (int a = 0; a < 3; ++a) {
+            if (!(w[DC_A_HALF + a] > 0.0)) return "distractor asset blob: DC_A_HALF (half extents) must be positive";
+            if (!(w[DC_A_RGB + a] >= 0.0 && w[DC_A_RGB + a] <= 1.0)) return "distractor asset blob: DC_A_RGB must lie in [0, 1]";
+        }
     }
     return nullptr;
 }

@@ -6,6 +6,7 @@
 #include "kuka_state.cuh"
 #include "kuka_device.cuh"
 #include "distractor_core.h"
+#include "render_core.h"
 
 // Trace capacity: T (action_repeat + 5) micro-steps per env -- at 4096 envs x 128 steps x (1 + 5) that is 201 MB.  The arm's 500 settle
 // micro-steps are one fixed trajectory per handle (`settle`).
@@ -17,6 +18,11 @@ struct DistDev {
     float4* settle;      // [500][4] the arm's settle trajectory
     size_t cap;          // micro-steps per env the trace holds
     DcAssets<float> A;
+};
+// The host's view of a handle's bodies: DistDev (distractor_kernel's parameter, unchanged) plus the per-type drawing table that
+// srl_sim_render's list kernel reads.
+struct DistHost : DistDev {
+    SrlBodyLooks looks;
 };
 
 namespace {
@@ -172,10 +178,11 @@ int dist_alloc(srl_sim* s, const void* blob, size_t bytes, float4** settle) {
     if (s->dist) { srl_set_error("set_distractors: already set"); return 1; }
     if (!blob) { srl_set_error("set_distractors: null asset blob"); return 1; }
     if (const char* err = dc_blob_error((const double*)blob, bytes)) { srl_set_error("set_distractors: %s", err); return 1; }
-    DistDev* g = new DistDev();
+    DistHost* g = new DistHost();
     memset(g, 0, sizeof(*g));
     s->dist = g;   // freed by kuka_free, also when srl_sim_set_distractors fails after this point
     dc_assets_from_blob((const double*)blob, g->A);
+    srl_body_looks((const double*)blob, g->looks);
     const size_t N = (size_t)s->n;
     SRL_CUDA_OK(cudaMalloc(&g->body, N * DC_NBODY * DC_B_WORDS * sizeof(float))); SRL_CUDA_OK(cudaMemset(g->body, 0, N * DC_NBODY * DC_B_WORDS * sizeof(float)));
     SRL_CUDA_OK(cudaMalloc(&g->touch, N * 2 * sizeof(uint32_t))); SRL_CUDA_OK(cudaMemset(g->touch, 0, N * 2 * sizeof(uint32_t)));
@@ -208,9 +215,15 @@ int dist_advance(srl_sim* s, const double* draws, cudaStream_t st) {
 void dist_free(srl_sim* s) {
     if (DistDev* g = s->dist) {
         cudaFree(g->body); cudaFree(g->touch); cudaFree(g->trace); cudaFree(g->trace_len); cudaFree(g->settle);
-        delete g;
+        delete static_cast<DistHost*>(g);
         s->dist = nullptr;
     }
+}
+
+const float* dist_render_bodies(const srl_sim* s, SrlBodyLooks* looks) {
+    if (!s->dist) return nullptr;
+    *looks = static_cast<const DistHost*>(s->dist)->looks;
+    return s->dist->body;
 }
 
 // SRL_F_DISTRACTORS and SRL_F_DISTRACTOR_TOUCH of kuka_get_state: zeros for a handle without bodies

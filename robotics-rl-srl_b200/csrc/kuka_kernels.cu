@@ -609,9 +609,11 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
 }
 
 // Scene primitives of every env for srl_sim_render (render_core.h): one thread per env recomputes the joint frames of the stored
-// configuration (the link states in HBM are only the two the env logic reads) and lists the primitives.
+// configuration (the link states in HBM are only the two the env logic reads) and lists the primitives, then the env's distractor bodies
+// when the handle has them (`bodies`: [N][DC_NBODY][DC_B_WORDS], written by distractor_kernel earlier on the same stream).
 template <bool TWOB>
-__global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, float* __restrict__ prims, int* __restrict__ counts) {
+__global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, const float* __restrict__ bodies, const __grid_constant__ SrlBodyLooks looks,
+                                  float* __restrict__ prims, int* __restrict__ counts) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const KukaParams& P = d.P;
@@ -639,7 +641,9 @@ __global__ void kuka_prims_kernel(const __grid_constant__ KukaDev d, int n, floa
     K.glider_z = P.glider_z; K.disc_r = P.disc_r; K.disc_z0 = P.disc_z0; K.disc_z1 = P.disc_z1; K.stack_r = P.stack_r; K.stack_top = P.stack_top;
     K.two_buttons = TWOB ? 1 : 0;
     SrlPrim* out = reinterpret_cast<SrlPrim*>(prims + (size_t)i * SRL_MAX_PRIMS * SRL_PRIM_WORDS);
-    counts[i] = srl_kuka_scene(K, jp, sph, ns, e.bbx, e.bby, e.bbz, e.qb, e.bb2x, e.bb2y, P.btn_base[2], e.qb2, out);
+    int np = srl_kuka_scene(K, jp, sph, ns, e.bbx, e.bby, e.bbz, e.qb, e.bb2x, e.bb2y, P.btn_base[2], e.qb2, out);
+    if (bodies) np = srl_distractor_prims(looks, bodies + (size_t)i * DC_NBODY * DC_B_WORDS, np, out);
+    counts[i] = np;
 }
 
 // ---- host side -------------------------------------------------------------------------------
@@ -864,8 +868,10 @@ int kuka_set_distractors(srl_sim* s, const void* blob, size_t bytes) {
 int kuka_render_prims(srl_sim* s, float* prims, int* counts, cudaStream_t st) {
     KukaDev* d = s->kuka;
     const int grid = (s->n + 63) / 64;
-    if (d->P.two_buttons) kuka_prims_kernel<true><<<grid, 64, 0, st>>>(*d, s->n, prims, counts);
-    else kuka_prims_kernel<false><<<grid, 64, 0, st>>>(*d, s->n, prims, counts);
+    SrlBodyLooks looks = {};
+    const float* bodies = dist_render_bodies(s, &looks);
+    if (d->P.two_buttons) kuka_prims_kernel<true><<<grid, 64, 0, st>>>(*d, s->n, bodies, looks, prims, counts);
+    else kuka_prims_kernel<false><<<grid, 64, 0, st>>>(*d, s->n, bodies, looks, prims, counts);
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }

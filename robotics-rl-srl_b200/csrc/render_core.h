@@ -4,7 +4,7 @@
 // What the reference does: `render(mode='rgb_array')` asks PyBullet's TinyRenderer for a 224 x 224 frame of the scene through
 // computeViewMatrixFromYawPitchRoll / computeProjectionMatrixFOV / getCameraImage (environments/kuka_gym/kuka_button_gym_env.py:370-420,
 // environments/mobile_robot/mobile_robot_env.py:287-334), and `srl_model="raw_pixels"` returns that frame as the observation.
-// What this is: a ray-caster of ANALYTIC primitives -- plane, sphere, capsule, upright cylinder, yaw-rotated box -- with ambient +
+// What this is: a ray-caster of ANALYTIC primitives -- plane, sphere, capsule, upright cylinder, yaw-rotated box, fully rotated box -- with ambient +
 // Lambert shading, through the same pinhole camera.  The meshes and textures TinyRenderer draws (pybullet_data: kuka_iiwa/meshes, table,
 // racecar, plane checker) are absent from the reference checkout and from this image, so the arm is drawn as capsules between its joint
 // frames plus its collision spheres, the table / walls as boxes, the buttons / targets as the z-extruded discs their collada meshes are:
@@ -13,6 +13,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include "distractor_core.h"
 
 #if defined(__CUDACC__)
 #define SRL_RHD __host__ __device__ __forceinline__
@@ -21,8 +22,12 @@
 #endif
 
 #define SRL_PRIM_WORDS 16
-#define SRL_MAX_PRIMS 40
-enum { SRL_PRIM_PLANE = 0, SRL_PRIM_SPHERE = 1, SRL_PRIM_CAPSULE = 2, SRL_PRIM_CYL = 3, SRL_PRIM_BOX = 4 };
+#define SRL_MAX_PRIMS 48
+enum { SRL_PRIM_PLANE = 0, SRL_PRIM_SPHERE = 1, SRL_PRIM_CAPSULE = 2, SRL_PRIM_CYL = 3, SRL_PRIM_BOX = 4, SRL_PRIM_OBOX = 5 };
+// the single-button Kuka scene (plane, table, 4 legs, 2 button, 8 arm capsules, 4 gripper capsules, 11 gripper spheres) plus every
+// distractor body of KukaRandButton must fit one list
+#define SRL_KUKA_ONE_BUTTON_PRIMS 31
+static_assert(SRL_KUKA_ONE_BUTTON_PRIMS + DC_NBODY <= SRL_MAX_PRIMS, "a KukaRandButton scene with all its bodies must fit SRL_MAX_PRIMS");
 
 // One primitive = 16 floats: type, 11 geometry words, r g b, pad.
 //   PLANE   a0 = z, a1 = checker period (0: plain), a2..4 = second colour of the checker
@@ -30,6 +35,7 @@ enum { SRL_PRIM_PLANE = 0, SRL_PRIM_SPHERE = 1, SRL_PRIM_CAPSULE = 2, SRL_PRIM_C
 //   CAPSULE a0..2 end 0, a3..5 end 1, a6 radius
 //   CYL     a0 cx, a1 cy, a2 z0, a3 z1, a4 radius            (upright, capped)
 //   BOX     a0..2 centre, a3..5 half extents, a6 cos, a7 sin  (rotated about z)
+//   OBOX    a0..2 centre, a3..5 half extents, a6..9 unit quaternion x y z w (any rotation; q and -q draw the same bytes)
 struct SrlPrim { float type, a[11], r, g, b, pad; };
 
 // pixel (x, y) (row 0 = top) looks along fwd + u right + v up with u = ub + su (x + 0.5), v = vb - sv (y + 0.5)
@@ -56,6 +62,11 @@ SRL_RHD void srl_prim_cyl(SrlPrim& p, float cx, float cy, float z0, float z1, fl
 SRL_RHD void srl_prim_box(SrlPrim& p, float cx, float cy, float cz, float hx, float hy, float hz, float yaw_cos, float yaw_sin, float r, float g, float b) {
     srl_prim_set(p, SRL_PRIM_BOX, r, g, b);
     p.a[0] = cx; p.a[1] = cy; p.a[2] = cz; p.a[3] = hx; p.a[4] = hy; p.a[5] = hz; p.a[6] = yaw_cos; p.a[7] = yaw_sin;
+}
+SRL_RHD void srl_prim_obox(SrlPrim& p, const float* c, const float* half, const float* quat, float r, float g, float b) {
+    srl_prim_set(p, SRL_PRIM_OBOX, r, g, b);
+    for (int i = 0; i < 3; ++i) { p.a[i] = c[i]; p.a[3 + i] = half[i]; }
+    for (int i = 0; i < 4; ++i) p.a[6 + i] = quat[i];
 }
 SRL_RHD void srl_prim_plane(SrlPrim& p, float z, float checker, float r, float g, float b) {
     srl_prim_set(p, SRL_PRIM_PLANE, r, g, b);
@@ -93,6 +104,21 @@ SRL_RHD void srl_camera_setup(const float* target, float distance, float yaw_deg
     c.vb = th; c.sv = 2.f * th / (float)H;
 }
 
+// ---- rotation by a unit quaternion q = (x y z w) and by its inverse, v' = v + w t + u x t with u = (x y z), t = 2 u x v (for the inverse
+//      u -> -u).  Every product pairs two components of q, so q and -q give the same bits.
+SRL_RHD void srl_quat_rotate(const float* q, const float* v, float* o) {
+    const float t[3] = {2.f * (q[1] * v[2] - q[2] * v[1]), 2.f * (q[2] * v[0] - q[0] * v[2]), 2.f * (q[0] * v[1] - q[1] * v[0])};
+    o[0] = v[0] + q[3] * t[0] + (q[1] * t[2] - q[2] * t[1]);
+    o[1] = v[1] + q[3] * t[1] + (q[2] * t[0] - q[0] * t[2]);
+    o[2] = v[2] + q[3] * t[2] + (q[0] * t[1] - q[1] * t[0]);
+}
+SRL_RHD void srl_quat_rotate_inv(const float* q, const float* v, float* o) {
+    const float t[3] = {2.f * (v[1] * q[2] - v[2] * q[1]), 2.f * (v[2] * q[0] - v[0] * q[2]), 2.f * (v[0] * q[1] - v[1] * q[0])};
+    o[0] = v[0] + q[3] * t[0] + (t[1] * q[2] - t[2] * q[1]);
+    o[1] = v[1] + q[3] * t[1] + (t[2] * q[0] - t[0] * q[2]);
+    o[2] = v[2] + q[3] * t[2] + (t[0] * q[1] - t[1] * q[0]);
+}
+
 // ---- per-camera prepared form of a primitive: everything of the intersection arithmetic that does not depend on the pixel ----------------
 //   PLANE   g0 = z - eye_z
 //   SPHERE  g0..2 = eye - centre, g3 = |eye - centre|^2 - r^2
@@ -100,6 +126,9 @@ SRL_RHD void srl_camera_setup(const float* target, float distance, float yaw_deg
 //           g9 = oa.oa - r^2, g10 = |eye - end1|^2 - r^2                (a zero-length capsule is prepared as the SPHERE it is)
 //   CYL     g0, g1 = eye.xy - centre.xy, g2 = g0^2 + g1^2 - r^2, g3 = z0 - eye_z, g4 = z1 - eye_z, g5 = r^2
 //   BOX     g0..2 = eye - centre in the box frame, g3..5 = half extents, g6 = cos, g7 = sin
+//   OBOX    g0..2 = eye - centre in the box frame, g3..5 = half extents, g6..9 = the quaternion.  The ray is rotated into the box frame per
+//           pixel (about 20 FMA) rather than kept as two prescaled axes plus a cross product: it fits g[11] with a word to spare, and the
+//           slab test then reads the same words (eye in the box frame, half extents) as BOX's, so both share it.
 // u0..v1: the screen-space bound the CUDA tile test reads (filled by the caller; the CPU checker does not cull).
 struct SrlPrep { float type, g[11], u0, u1, v0, v1; };
 
@@ -129,6 +158,10 @@ SRL_RHD void srl_prepare(const float* eye, const SrlPrim& p, SrlPrep& q) {
     } else if (type == SRL_PRIM_CYL) {
         const float ox = eye[0] - p.a[0], oy = eye[1] - p.a[1];
         q.g[0] = ox; q.g[1] = oy; q.g[2] = ox * ox + oy * oy - p.a[4] * p.a[4]; q.g[3] = p.a[2] - eye[2]; q.g[4] = p.a[3] - eye[2]; q.g[5] = p.a[4] * p.a[4];
+    } else if (type == SRL_PRIM_OBOX) {
+        const float o[3] = {eye[0] - p.a[0], eye[1] - p.a[1], eye[2] - p.a[2]};
+        srl_quat_rotate_inv(p.a + 6, o, q.g);
+        for (int i = 3; i < 10; ++i) q.g[i] = p.a[i];
     } else {
         const float cs = p.a[6], sn = p.a[7], px = eye[0] - p.a[0], py = eye[1] - p.a[1];
         q.g[0] = cs * px + sn * py; q.g[1] = -sn * px + cs * py; q.g[2] = eye[2] - p.a[2];
@@ -143,6 +176,8 @@ SRL_RHD bool srl_sphere_t(float b, float cc, float& t) {          // b = (eye - 
     t = -b - sqrtf(h);
     return t > 1e-4f;
 }
+// OBOX = false compiles a caller that never sees an oriented box (the CUDA raster kernel for lists without distractor bodies) without its code
+template <bool OBOX = true>
 SRL_RHD bool srl_hit_t(const SrlPrep& q, const float* d, float& t) {
     const int type = (int)q.type;
     const float* g = q.g;
@@ -190,7 +225,9 @@ SRL_RHD bool srl_hit_t(const SrlPrep& q, const float* d, float& t) {
         return true;
     }
     // box: slabs in the box frame
-    const float ld[3] = {g[6] * d[0] + g[7] * d[1], -g[7] * d[0] + g[6] * d[1], d[2]};
+    float ld[3];
+    if (OBOX && type == SRL_PRIM_OBOX) srl_quat_rotate_inv(g + 6, d, ld);
+    else { ld[0] = g[6] * d[0] + g[7] * d[1]; ld[1] = -g[7] * d[0] + g[6] * d[1]; ld[2] = d[2]; }
     float tn = -1e30f, tf = 1e30f;
     for (int k = 0; k < 3; ++k) {
         if (fabsf(ld[k]) < 1e-12f) { if (fabsf(g[k]) > g[3 + k]) return false; continue; }
@@ -205,7 +242,16 @@ SRL_RHD bool srl_hit_t(const SrlPrep& q, const float* d, float& t) {
     return true;
 }
 
+// the face of a box (half extents h) a point l in the box frame lies on: the axis whose slab it is closest to leaving, as a signed unit vector
+SRL_RHD void srl_box_face(const float* l, const float* h, float* ln) {
+    int axis = 0; float out = fabsf(l[0]) - h[0], la = l[0];          // la = l[axis], kept without indexing by a run-time axis (local memory)
+    for (int k = 1; k < 3; ++k) { const float o = fabsf(l[k]) - h[k]; if (o > out) { out = o; axis = k; la = l[k]; } }
+    const float sg = la < 0.f ? -1.f : 1.f;
+    ln[0] = axis == 0 ? sg : 0.f; ln[1] = axis == 1 ? sg : 0.f; ln[2] = axis == 2 ? sg : 0.f;
+}
+
 // Outward unit normal of primitive p at the surface point P.
+template <bool OBOX = true>
 SRL_RHD void srl_normal_at(const SrlPrim& p, const float* P, float* n) {
     const int type = (int)p.type;
     n[0] = 0.f; n[1] = 0.f; n[2] = 1.f;
@@ -223,11 +269,15 @@ SRL_RHD void srl_normal_at(const SrlPrim& p, const float* P, float* n) {
     } else if (type == SRL_PRIM_BOX) {
         const float cs = p.a[6], sn = p.a[7], px = P[0] - p.a[0], py = P[1] - p.a[1];
         const float l[3] = {cs * px + sn * py, -sn * px + cs * py, P[2] - p.a[2]};
-        int axis = 0; float out = fabsf(l[0]) - p.a[3];                   // the face the point lies on: the axis whose slab it is closest to leaving
-        for (int k = 1; k < 3; ++k) { const float o = fabsf(l[k]) - p.a[3 + k]; if (o > out) { out = o; axis = k; } }
-        const float sg = l[axis] < 0.f ? -1.f : 1.f;
-        const float ln[3] = {axis == 0 ? sg : 0.f, axis == 1 ? sg : 0.f, axis == 2 ? sg : 0.f};
+        float ln[3];
+        srl_box_face(l, p.a + 3, ln);
         n[0] = cs * ln[0] - sn * ln[1]; n[1] = sn * ln[0] + cs * ln[1]; n[2] = ln[2];
+    } else if (OBOX && type == SRL_PRIM_OBOX) {
+        const float w[3] = {P[0] - p.a[0], P[1] - p.a[1], P[2] - p.a[2]};
+        float l[3], ln[3];
+        srl_quat_rotate_inv(p.a + 6, w, l);
+        srl_box_face(l, p.a + 3, ln);
+        srl_quat_rotate(p.a + 6, ln, n);
     }
 }
 
@@ -235,6 +285,7 @@ SRL_RHD void srl_normal_at(const SrlPrim& p, const float* P, float* n) {
 // TOP of the image (getCameraImage).  The CUDA kernel passes the subset whose screen bound reaches the pixel's neighbourhood; the CPU checker
 // passes all of them.  `prep[k]` is srl_prepare(c.eye, prims[k]).
 SRL_RHD unsigned long long srl_prim_mask_all(int np) { return np >= 64 ? ~0ull : ((1ull << np) - 1ull); }
+template <bool OBOX = true>
 SRL_RHD void srl_render_pixel(const SrlCam& c, const SrlPrep* prep, const SrlPrim* prims, unsigned long long mask, int x, int y, uint8_t* rgb) {
     const float u = c.ub + c.su * ((float)x + 0.5f);
     const float v = c.vb - c.sv * ((float)y + 0.5f);
@@ -251,14 +302,14 @@ SRL_RHD void srl_render_pixel(const SrlCam& c, const SrlPrep* prep, const SrlPri
 #endif
         mask &= mask - 1ull;
         float t = 0.f;
-        if (srl_hit_t(prep[k], d, t) && t < best) { best = t; win = k; }
+        if (srl_hit_t<OBOX>(prep[k], d, t) && t < best) { best = t; win = k; }
     }
     float shade = 1.f, col[3] = {0.84f, 0.89f, 0.95f};                 // background (above the horizon)
     if (win >= 0) {
         const SrlPrim& p = prims[win];
         const float P[3] = {c.eye[0] + best * d[0], c.eye[1] + best * d[1], c.eye[2] + best * d[2]};
         float n[3];
-        srl_normal_at(p, P, n);
+        srl_normal_at<OBOX>(p, P, n);
         col[0] = p.r; col[1] = p.g; col[2] = p.b;
         if ((int)p.type == SRL_PRIM_PLANE && p.a[1] > 0.f) {
             const int ix = (int)floorf(P[0] / p.a[1]), iy = (int)floorf(P[1] / p.a[1]);
@@ -312,6 +363,31 @@ SRL_RHD int srl_kuka_scene(const SrlKukaSceneConst& K, const float* joint_p, con
     srl_prim_capsule(out[n++], joint_p + 21, joint_p + 30, 0.02f, 0.15f, 0.15f, 0.15f);
     srl_prim_capsule(out[n++], joint_p + 30, joint_p + 33, 0.012f, 0.15f, 0.15f, 0.15f);
     for (int k = 0; k < nsph && n < SRL_MAX_PRIMS; ++k) srl_prim_sphere(out[n++], sph + 4 * k, sph[4 * k + 3], 0.2f, 0.2f, 0.2f);
+    return n;
+}
+
+// KukaRandButton's distractor bodies: per object type the drawing words of the asset blob (distractor_core.h DC_A_SHAPE / DC_A_HALF /
+// DC_A_RGB; srl_sim/model.py: distractor_blob), checked by dc_blob_error.
+struct SrlBodyLooks { float shape[DC_NTYPE], half[DC_NTYPE][3], rgb[DC_NTYPE][3]; };
+SRL_RHD void srl_body_looks(const double* blob, SrlBodyLooks& L) {
+    for (int t = 0; t < DC_NTYPE; ++t) {
+        const double* w = blob + t * DC_TYPE_WORDS;
+        L.shape[t] = (float)w[DC_A_SHAPE];
+        for (int i = 0; i < 3; ++i) { L.half[t][i] = (float)w[DC_A_HALF + i]; L.rgb[t][i] = (float)w[DC_A_RGB + i]; }
+    }
+}
+
+// The present bodies of one env (B: DC_NBODY x DC_B_WORDS, distractor_core.h) appended to a scene list of n primitives: shape 0 a box of the
+// type's half extents at the body's pose, shape 1 a sphere of radius half[0].  They come after the scene, and the nearest-hit search takes
+// a later primitive only when it is strictly nearer, so the pixels no body covers keep the bytes they have without bodies.
+SRL_RHD int srl_distractor_prims(const SrlBodyLooks& L, const float* B, int n, SrlPrim* out) {
+    for (int k = 0; k < DC_NBODY && n < SRL_MAX_PRIMS; ++k) {
+        const float* b = B + k * DC_B_WORDS;
+        if (b[DC_B_PRESENT] == 0.f) continue;
+        const int t = (int)b[DC_B_TYPE];
+        if (L.shape[t] == 1.f) srl_prim_sphere(out[n++], b + DC_B_P, L.half[t][0], L.rgb[t][0], L.rgb[t][1], L.rgb[t][2]);
+        else srl_prim_obox(out[n++], b + DC_B_P, L.half[t], b + DC_B_Q, L.rgb[t][0], L.rgb[t][1], L.rgb[t][2]);
+    }
     return n;
 }
 

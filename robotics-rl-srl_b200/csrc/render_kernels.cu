@@ -1,7 +1,7 @@
 // Image observations for the batched simulator (SURVEY.md 8(f).4): one launch builds every env's primitive list from its state, one launch
 // ray-casts all frames.  Per-pixel arithmetic and the scene lists live in render_core.h (shared with the CPU checker).
 //
-// Layout: the primitive lists are [N][SRL_MAX_PRIMS][16 floats] in HBM (2.5 KB per env), and so are their per-camera prepared forms (the
+// Layout: the primitive lists are [N][SRL_MAX_PRIMS][16 floats] in HBM (3 KB per env), and so are their per-camera prepared forms (the
 // pixel-independent part of the intersection arithmetic + a screen-space bound).  The raster kernel runs one CTA of 32 x 16 pixels per
 // (tile, env): it stages the env's prepared list in shared memory once, each warp keeps the primitives whose bound reaches its 8 x 8 pixel
 // block, and the RGB bytes go out row-major -- a 224 x 224 frame is 98 tiles, 4096 envs are 401 k CTAs, 617 MB of output per call.
@@ -70,6 +70,19 @@ __device__ __forceinline__ bool prim_rect(const SrlCam& c, const SrlPrim& p, Scr
         }
         return ok;
     }
+    if (type == SRL_PRIM_OBOX) {                          // its 8 rotated corners, padded as BOX's
+        bool ok = true;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float l[3] = {((k & 1) ? 1.f : -1.f) * (p.a[3] * 1.001f + 1e-4f), ((k & 2) ? 1.f : -1.f) * (p.a[4] * 1.001f + 1e-4f),
+                                ((k & 4) ? 1.f : -1.f) * (p.a[5] * 1.001f + 1e-4f)};
+            float w[3];
+            srl_quat_rotate(p.a + 6, l, w);
+            cam_space(c, p.a[0] + w[0], p.a[1] + w[1], p.a[2] + w[2], q);
+            ok = rect_point(r, q) && ok;
+        }
+        return ok;
+    }
     return false;
 }
 
@@ -93,7 +106,8 @@ __global__ void prepare_kernel(const float* __restrict__ prims, const int* __res
 // when the frame geometry allows.  grid = (tiles across, tiles down, envs).
 #define SRL_TILE_W 32
 #define SRL_TILE_H 16
-template <bool CULL>
+// BODIES: the lists may hold oriented boxes (a Kuka handle with distractor bodies); the kernel for the other lists leaves their code out.
+template <bool CULL, bool BODIES>
 __global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, SrlCam cam,
                                                       int W, int H, uint8_t* __restrict__ rgb) {
     static_assert(SRL_MAX_PRIMS <= 64, "the kept set is a 64-bit mask");
@@ -133,7 +147,7 @@ __global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ p
         const int ly = by + (lane >> 3) + 4 * r, y = y0 + ly;
         if (x < W && y < H) {
             uint8_t px[3];
-            srl_render_pixel(cam, sq, mine, mask, x, y, px);
+            srl_render_pixel<BODIES>(cam, sq, mine, mask, x, y, px);
             if (words) { tile[ly][3 * lx] = px[0]; tile[ly][3 * lx + 1] = px[1]; tile[ly][3 * lx + 2] = px[2]; }
             else {
                 uint8_t* o = rgb + ((size_t)env * H * W + (size_t)y * W + x) * 3;
@@ -167,11 +181,18 @@ int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint
     prepare_kernel<<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, c, s->n, s->render_prep);
     const bool no_cull = getenv("SRL_RENDER_NO_CULL") != nullptr;       // debugging aid: the block test is conservative, so both paths give the same bytes (tests/test_render_gpu.py)
     const size_t per_env = (size_t)SRL_MAX_PRIMS * SRL_PRIM_WORDS;
+    const bool bodies = s->dist != nullptr;
     for (int e0 = 0; e0 < s->n; e0 += 65535) {                           // grid.z is limited to 65535
         const dim3 grid((width + SRL_TILE_W - 1) / SRL_TILE_W, (height + SRL_TILE_H - 1) / SRL_TILE_H, min(65535, s->n - e0));
         uint8_t* out = rgb + (size_t)e0 * height * width * 3;
-        if (no_cull) raster_kernel<false><<<grid, 256, 0, st>>>(s->render_prims + e0 * per_env, s->render_prep + e0 * per_env, s->render_counts + e0, c, width, height, out);
-        else raster_kernel<true><<<grid, 256, 0, st>>>(s->render_prims + e0 * per_env, s->render_prep + e0 * per_env, s->render_counts + e0, c, width, height, out);
+        const float* pr = s->render_prims + e0 * per_env; const float* pp = s->render_prep + e0 * per_env; const int* cn = s->render_counts + e0;
+        if (bodies) {
+            if (no_cull) raster_kernel<false, true><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
+            else raster_kernel<true, true><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
+        } else {
+            if (no_cull) raster_kernel<false, false><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
+            else raster_kernel<true, false><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
+        }
     }
     SRL_CUDA_OK(cudaGetLastError());
     s->launches += 3;

@@ -5,7 +5,9 @@ kicked at env step 10 (:58-68,117-127).  They are simulated with ``distractors=T
 placements use the env's own ``np_random`` draws like the reference, the object types the global ``np.random``
 like the reference, and the kick direction the library's counter-based stream (the reference's global, unseeded
 draw is not reproducible anyway).  The bodies never push the arm back, so observations, rewards and done flags are
-the same with and without them; they show in ``getDistractors()``.
+the same with and without them; they show in ``getDistractors()`` and in every rendered frame (``srl_model="raw_pixels"``
+observations, ``render()``, ``multi_view`` and the frames ``record_data=True`` saves), the duck, the brick and the cube as the
+boxes the asset blob declares, the sphere as a ball (``srl_sim.model.distractor_blob``).
 Everything else -- MAX_STEPS, the env RNG draws of reset() -- is identical to KukaButtonGymEnv.
 """
 from .kuka_button_gym_env import *  # noqa: F401,F403

@@ -82,7 +82,8 @@ class BatchedSRLVecEnv(object):
                 cfg[k] = env_kwargs[k]
         self.sim = self.backend.make_sim(env_id, self.num_envs, seed=seed, model_blob=blob, **cfg)
         if self.distractors:
-            # kuka_rand_button_gym_env.py:58-68: random objects around the button and a kicked sphere (one-way coupled: the arm's outputs do not change)
+            # kuka_rand_button_gym_env.py:58-68: random objects around the button and a kicked sphere (one-way coupled: the arm's outputs do not
+            # change); srl_sim_render draws them, so raw_pixels observations and render_tensors() show them
             from .model import distractor_blob
             self.sim.set_distractors(distractor_blob())
         self.is_discrete = bool(cfg["is_discrete"])
