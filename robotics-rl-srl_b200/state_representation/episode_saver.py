@@ -15,8 +15,9 @@ with S = recorded transitions and E = episodes: row k of every S-array describes
 episode is the post-reset state, ``episode_starts`` True), and the terminal state of an episode is not recorded.
 
 Internally it is a table writer: rows accumulate in a ``_Table`` of typed columns, an episode is a row range, and the npz files are
-re-written from the table whenever an episode closes.  The simulator has no rasteriser (SURVEY section 8(f), item 4), so a ``None``
-observation contributes its frame NAME only (``<name>/record_000/frame000000``, the path the reference would have written);
+re-written from the table whenever an episode closes.  A ``None`` observation contributes its frame NAME only
+(``<name>/record_000/frame000000``, the path the reference would have written); an image array is written with cv2, and an already
+encoded JPEG file (``bytes``, or a pair of them for two cameras: ``srl_sim.jpeg.encode_jpeg``) is written as it is;
 ``learn_states`` (the SRL server round trip) is out of scope.
 """
 import json
@@ -99,8 +100,18 @@ class EpisodeSaver(object):
         return "record_{:03d}".format(self.episode_idx)
 
     def _frame(self, observation):
-        """Name of the frame of the current (episode, step); the image itself is written only when an array is supplied."""
+        """Name of the frame of the current (episode, step); the image itself is written only when an array or encoded JPEG bytes are
+        supplied.  ``bytes`` is a finished file (``srl_sim.jpeg.encode_jpeg``), written as ``<frame>.jpg``; a pair of ``bytes`` (two
+        cameras) is written as ``<frame>_1.jpg`` and ``<frame>_2.jpg``, the reference's multi-view names."""
         rel = "{}/{}/frame{:06d}".format(self.name, self.episode_folder, self.episode_step)
+        if isinstance(observation, bytes) or (isinstance(observation, (tuple, list)) and observation and
+                                              all(isinstance(o, bytes) for o in observation)):
+            files = [observation] if isinstance(observation, bytes) else list(observation)
+            suffixes = [""] if len(files) == 1 else ["_{}".format(i + 1) for i in range(len(files))]
+            for data, suffix in zip(files, suffixes):
+                with open("{}{}{}.jpg".format(self.path, rel, suffix), "wb") as f:
+                    f.write(data)
+            return rel
         if observation is not None and getattr(observation, "ndim", 0) == 3:
             import cv2
             cv2.imwrite("{}{}.jpg".format(self.path, rel), cv2.cvtColor(observation[:, :, :3], cv2.COLOR_BGR2RGB))
