@@ -31,6 +31,28 @@
 #define KC_RSQRT(x) (1.0f / sqrtf(x))
 #endif
 
+// Diagnostic build (scripts/build_variant.sh phases -DKK_PHASES, scripts/kuka_phase_timing.py): clock() accumulators per phase of the
+// micro-step loop, in registers, stored per env slot at the end of the launch.  Separate from KK_TIMING, whose convergence probe adds
+// instructions to every sweep row.  KK_PH(clk, k) charges the cycles since the previous mark to phase k; without KK_PHASES it is empty.
+// 32-bit accumulators (a slot runs ~10^7 cycles per launch): half the registers of clock64() ones, so the 21 marks add fewer spills.
+// The fast sweeps are charged to one of two phases, by the copy of the loop the warp ran (no lane
+// watching a contact, or the watch copy); `nwatch` counts the physics steps of the slot that ran the watch copy.
+enum {
+    KK_PH_KIN_LOCAL = 0, KK_PH_KIN_CHAIN, KK_PH_KIN_BODY, KK_PH_KIN_COLLECT,              // kinematics + collision (kc_kinematics)
+    KK_PH_IK_BUILD, KK_PH_IK_SOLVE,                                                     // J, error, J^T J, J^T e / the 7x7 solve
+    KK_PH_DYN_D1, KK_PH_DYN_D2, KK_PH_DYN_D3, KK_PH_DYN_D4, KK_PH_DYN_D5, KK_PH_DYN_D6, KK_PH_DYN_D7,   // kc_dynamics (+ loading M, bias)
+    KK_PH_CHOL,                                                                         // Cholesky + M^-1
+    KK_PH_SETUP, KK_PH_ROWS, KK_PH_EULER,                                               // v0 + motor / limit set-up, contact rows + scaling, Euler
+    KK_PH_FAST_QUIET, KK_PH_FAST_WATCH, KK_PH_GENERAL, KK_PH_ENV, KK_NPH
+};
+#if defined(KK_PHASES) && defined(__CUDACC__)
+struct KkPhaseClock { unsigned last; unsigned acc[KK_NPH]; unsigned nwatch; };
+#define KK_PH(clk, k) do { if (clk) { const unsigned t_ = (unsigned)clock(); (clk)->acc[k] += t_ - (clk)->last; (clk)->last = t_; } } while (0)
+#else
+struct KkPhaseClock { long long dummy; };
+#define KK_PH(clk, k) do { (void)(clk); } while (0)
+#endif
+
 #define KC_G 4               // lanes per env
 #define KC_BS 53             // per-body record stride in words (odd: 4 lanes on 4 different bodies hit 4 different banks)
 #define KC_CS 25             // per-body constant record stride (odd)
@@ -127,6 +149,14 @@ KC_F int kc_parent(int i) { return i == 0 ? -1 : i == 10 ? 7 : i - 1; }
 KC_F bool kc_anc(int i, int j) { return (i == j) || (i <= 7 && i < j) || (i == 8 && j == 9) || (i == 10 && j == 11); }
 // value k of a 12-vector held in registers by every lane, for the body u + 4 k of lane u (static register indices only)
 #define KC_SEL4(arr, k, u) ((u) == 0 ? (arr)[4 * (k)] : (u) == 1 ? (arr)[4 * (k) + 1] : (u) == 2 ? (arr)[4 * (k) + 2] : (arr)[4 * (k) + 3])
+// index of the lowest set bit of x != 0
+KC_F int kc_lowest_bit(unsigned x) {
+#if defined(__CUDA_ARCH__)
+    return __ffs(x) - 1;
+#else
+    return __builtin_ctz(x);
+#endif
+}
 
 // sphere vs upright finite cylinder (axis +z through (cx, cy), z in [z0, z1], radius R)
 KC_F void kc_sphere_cylinder(kc3 s, float r, float cx, float cy, float z0, float z1, float R, float& dist, kc3& n) {
@@ -157,49 +187,68 @@ struct KcKinIn {
 
 // ================================================================ kinematics ======================================================
 // Phase 1: local rotations of the lane's bodies.
+// The constant table and the scratch area are both shared memory: a table load that follows a scratch store in program order waits for
+// it.  So every phase loads its constants (and the scratch words it reads) ahead of its stores.
 template <class S>
 KC_F void kc_ph_local(const S& s, const float* tab, const KcKinIn& in, int u) {
+    float ax[KK_NB / KC_G][3], rot[KK_NB / KC_G][9];
+#pragma unroll
+    for (int k = 0; k < KK_NB / KC_G; ++k) {
+        const float* c = tab + (u + KC_G * k) * KC_CS;
+#pragma unroll
+        for (int t = 0; t < 3; ++t) ax[k][t] = c[KCB_AXIS + t];
+#pragma unroll
+        for (int t = 0; t < 9; ++t) rot[k][t] = c[KCB_ROT + t];
+    }
 #pragma unroll
     for (int k = 0; k < KK_NB / KC_G; ++k) {
         const int i = u + KC_G * k;
         const float qi = KC_SEL4(in.q, k, u);
         float sn, cs;
         sincosf(qi, &sn, &cs);
-        const float* c = tab + i * KC_CS;
-        const float t = 1.f - cs, ax = c[KCB_AXIS], ay = c[KCB_AXIS + 1], az = c[KCB_AXIS + 2];
-        const float Q[9] = {cs + t * ax * ax, t * ax * ay - sn * az, t * ax * az + sn * ay,
-                            t * ax * ay + sn * az, cs + t * ay * ay, t * ay * az - sn * ax,
-                            t * ax * az - sn * ay, t * ay * az + sn * ax, cs + t * az * az};
+        const float t = 1.f - cs, ax0 = ax[k][0], ay = ax[k][1], az = ax[k][2];
+        const float Q[9] = {cs + t * ax0 * ax0, t * ax0 * ay - sn * az, t * ax0 * az + sn * ay,
+                            t * ax0 * ay + sn * az, cs + t * ay * ay, t * ay * az - sn * ax0,
+                            t * ax0 * az - sn * ay, t * ay * az + sn * ax0, cs + t * az * az};
 #pragma unroll
         for (int r = 0; r < 3; ++r)
 #pragma unroll
             for (int cc = 0; cc < 3; ++cc)
-                s[i * KC_BS + KB_B + 3 * r + cc] = fmaf(c[KCB_ROT + 3 * r + 2], Q[6 + cc], fmaf(c[KCB_ROT + 3 * r + 1], Q[3 + cc], c[KCB_ROT + 3 * r] * Q[cc]));
+                s[i * KC_BS + KB_B + 3 * r + cc] = fmaf(rot[k][3 * r + 2], Q[6 + cc], fmaf(rot[k][3 * r + 1], Q[3 + cc], rot[k][3 * r] * Q[cc]));
     }
 }
 
-// Phase 2: the transform chain, one ROW of every world rotation (and one component of every origin) per lane; lane 3 idles.
+// Phase 2: the transform chain, one ROW of every world rotation (and one component of every origin) per lane; lane 3 idles.  The local
+// rotation and the origin offset of body i + 2 are loaded before the stores of body i (registers: static indices after unrolling).
 template <class S>
 KC_F void kc_ph_chain(const S& s, const float* tab, const KukaParams& P, int u) {
     if (u >= 3) return;
+    float B[KK_NB][9], O[KK_NB][3];
+#define KC_CHAIN_LOAD(j)                                                                  \
+    {                                                                                     \
+        _Pragma("unroll") for (int t = 0; t < 9; ++t) B[j][t] = s[(j) * KC_BS + KB_B + t]; \
+        _Pragma("unroll") for (int t = 0; t < 3; ++t) O[j][t] = tab[(j) * KC_CS + KCB_ORG + t]; \
+    }
+    KC_CHAIN_LOAD(0)
+    KC_CHAIN_LOAD(1)
     float R0 = u == 0 ? 1.f : 0.f, R1 = u == 1 ? 1.f : 0.f, R2 = u == 2 ? 1.f : 0.f;
     float p = u == 0 ? P.base[0] : u == 1 ? P.base[1] : P.base[2];
     float S0 = R0, S1 = R1, S2 = R2, sp = p;   // body 7: where the second finger restarts
 #pragma unroll
     for (int i = 0; i < KK_NB; ++i) {
+        if (i + 2 < KK_NB) KC_CHAIN_LOAD(i + 2)
         if (i == 10) { R0 = S0; R1 = S1; R2 = S2; p = sp; }
-        const float* c = tab + i * KC_CS;
-        p = fmaf(R2, c[KCB_ORG + 2], fmaf(R1, c[KCB_ORG + 1], fmaf(R0, c[KCB_ORG], p)));
-        const int b = i * KC_BS + KB_B;
-        const float n0 = fmaf(R2, s[b + 6], fmaf(R1, s[b + 3], R0 * s[b + 0]));
-        const float n1 = fmaf(R2, s[b + 7], fmaf(R1, s[b + 4], R0 * s[b + 1]));
-        const float n2 = fmaf(R2, s[b + 8], fmaf(R1, s[b + 5], R0 * s[b + 2]));
+        p = fmaf(R2, O[i][2], fmaf(R1, O[i][1], fmaf(R0, O[i][0], p)));
+        const float n0 = fmaf(R2, B[i][6], fmaf(R1, B[i][3], R0 * B[i][0]));
+        const float n1 = fmaf(R2, B[i][7], fmaf(R1, B[i][4], R0 * B[i][1]));
+        const float n2 = fmaf(R2, B[i][8], fmaf(R1, B[i][5], R0 * B[i][2]));
         R0 = n0; R1 = n1; R2 = n2;
         const int r = i * KC_BS + KB_R + 3 * u;
         s[r] = R0; s[r + 1] = R1; s[r + 2] = R2;
         s[i * KC_BS + KB_P + u] = p;
         if (i == 7) { S0 = R0; S1 = R1; S2 = R2; sp = p; }
     }
+#undef KC_CHAIN_LOAD
 }
 
 // Phase 3: world-frame quantities of the lane's bodies + collision candidates of the lane's spheres.
@@ -214,6 +263,8 @@ KC_F bool kc_ph_body(const S& s, const float* tab, const KukaParams& P, const Kc
         for (int t = 0; t < 9; ++t) R[t] = s[o + KB_R + t];
         const kc3 p = kc_ld3(s, o + KB_P);
         const float ax = c[KCB_AXIS], ay = c[KCB_AXIS + 1], az = c[KCB_AXIS + 2];
+        const float I0 = c[KCB_IC], I1 = c[KCB_IC + 1], I2 = c[KCB_IC + 2], I3 = c[KCB_IC + 3], I4 = c[KCB_IC + 4], I5 = c[KCB_IC + 5];
+        const float m = c[KCB_MASS];    // (all loads ahead of the stores)
         const kc3 a = kc_mk(fmaf(R[2], az, fmaf(R[1], ay, R[0] * ax)), fmaf(R[5], az, fmaf(R[4], ay, R[3] * ax)), fmaf(R[8], az, fmaf(R[7], ay, R[6] * ax)));
         const float mx = c[KCB_COM], my = c[KCB_COM + 1], mz = c[KCB_COM + 2];
         const kc3 cm = kc_mk(fmaf(R[2], mz, fmaf(R[1], my, fmaf(R[0], mx, p.x))), fmaf(R[5], mz, fmaf(R[4], my, fmaf(R[3], mx, p.y))),
@@ -222,7 +273,6 @@ KC_F bool kc_ph_body(const S& s, const float* tab, const KukaParams& P, const Kc
         kc_st3(s, o + KB_PV, kc_cross(p, a));
         kc_st3(s, o + KB_C, cm);
         // Iw = R Ic R^T
-        const float I0 = c[KCB_IC], I1 = c[KCB_IC + 1], I2 = c[KCB_IC + 2], I3 = c[KCB_IC + 3], I4 = c[KCB_IC + 4], I5 = c[KCB_IC + 5];
         float T[9];
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
@@ -240,7 +290,6 @@ KC_F bool kc_ph_body(const S& s, const float* tab, const KukaParams& P, const Kc
 #pragma unroll
         for (int t = 0; t < 6; ++t) s[o + KB_IW + t] = Iw[t];
         // spatial inertia about the world origin: m, h = m c, I_O = Iw + m (|c|^2 1 - c c^T)
-        const float m = c[KCB_MASS];
         s[o + KB_M] = m;
         kc_st3(s, o + KB_H, kc_scale(m, cm));
         s[o + KB_IO + 0] = fmaf(m, fmaf(cm.y, cm.y, cm.z * cm.z), Iw[0]);
@@ -259,8 +308,9 @@ KC_F bool kc_ph_body(const S& s, const float* tab, const KukaParams& P, const Kc
     float zmax_shapes = fmaxf(disc1, fmaxf(bz + P.stack_top, P.table_z));
     if (TWOB) zmax_shapes = fmaxf(zmax_shapes, fmaxf(disc21, b2z + P.stack_top));
     float zmin_body = 1e30f;
-#pragma unroll 1
-    for (int i = P.sph_min_body; i < KK_NB; ++i) zmin_body = fminf(zmin_body, s[i * KC_BS + KB_P + 2]);
+#pragma unroll
+    for (int i = 0; i < KK_NB; ++i)   // independent loads (a rolled loop waits for each)
+        if (i >= P.sph_min_body) zmin_body = fminf(zmin_body, s[i * KC_BS + KB_P + 2]);
     const bool near = zmin_body - P.sph_reach - zmax_shapes <= P.cdist;
     if (!near) return false;    // (the same value in the 4 lanes) no candidate is written, the collect phase is skipped
 #pragma unroll 1
@@ -308,9 +358,16 @@ KC_F bool kc_ph_body(const S& s, const float* tab, const KukaParams& P, const Kc
 template <bool TWOB, class S>
 KC_F void kc_ph_collect(const S& s, const float* tab, const KukaParams& P, int u) {
     if (u != 0) return;
+    // the candidate counts of all spheres first (independent loads), then a walk over the few spheres that have any, in sphere order
+    // (a walk that loads each count and branches on it waits for one shared-memory load per sphere)
+    unsigned has = 0u;
+#pragma unroll
+    for (int sidx = 0; sidx < KM_MAX_SPHERES; ++sidx)
+        if (sidx < P.nsph && s[KC_OFF_CAND + sidx * KC_CANDW] > 0.f) has |= 1u << sidx;
     int flags = 0, nc = 0;      // bit 0 button disc, 1 table, 2 any link of button 1, 3 any link of button 2
 #pragma unroll 1
-    for (int sidx = 0; sidx < P.nsph; ++sidx) {
+    for (; has != 0u; has &= has - 1u) {
+        const int sidx = kc_lowest_bit(has);
         const int cw = KC_OFF_CAND + sidx * KC_CANDW;
         int ncand = (int)s[cw];
         if (ncand > KC_CANDS) ncand = KC_CANDS;
@@ -323,9 +380,12 @@ KC_F void kc_ph_collect(const S& s, const float* tab, const KukaParams& P, int u
             if (TWOB) { if (shape == 1 || shape == 2) flags |= 4; if (shape >= 3) flags |= 8; }
             if (nc < P.max_contacts && nc < KK_MAXC) {
                 const int c = KC_OFF_CT + nc * KC_CTS;
-                s[c] = tab[KC_CONST_SPH + sidx * 5]; s[c + 1] = s[w]; s[c + 2] = s[w + 1];
+                float rec[KC_CTS];      // loaded whole, then stored
+                rec[0] = tab[KC_CONST_SPH + sidx * 5];
 #pragma unroll
-                for (int t = 0; t < 6; ++t) s[c + 3 + t] = s[w + 2 + t];
+                for (int t = 0; t < 8; ++t) rec[1 + t] = s[w + t];
+#pragma unroll
+                for (int t = 0; t < KC_CTS; ++t) s[c + t] = rec[t];
                 ++nc;
             }
         }
@@ -518,11 +578,14 @@ KC_F void kc_ph_rows(const S& s, const KukaParams& P, const float (&A)[KK_NB][KK
 // body records (COM of link 8, origin of link 6).
 #if defined(__CUDACC__)
 template <bool TWOB, class S>
-KC_F bool kc_kinematics(const S& s, const float* tab, const KukaParams& P, const KcKinIn& in, int u, unsigned gmask) {
+KC_F bool kc_kinematics(const S& s, const float* tab, const KukaParams& P, const KcKinIn& in, int u, unsigned gmask, KkPhaseClock* ph) {
     KC_RUN(kc_ph_local(s, tab, in, u));
+    KK_PH(ph, KK_PH_KIN_LOCAL);
     KC_RUN(kc_ph_chain(s, tab, P, u));
+    KK_PH(ph, KK_PH_KIN_CHAIN);
     const bool near = kc_ph_body<TWOB>(s, tab, P, in, u);
     __syncwarp(gmask);
+    KK_PH(ph, KK_PH_KIN_BODY);
     if (near) KC_RUN((kc_ph_collect<TWOB>(s, tab, P, u)));
     return near;
 }
@@ -540,16 +603,23 @@ KC_F bool kc_kinematics(const S& s, const float* tab, const KukaParams& P, const
 
 #if defined(__CUDACC__)
 template <class S>
-KC_F void kc_dynamics(const S& s, const KukaParams& P, const float* qd, int u, unsigned gmask) {
+KC_F void kc_dynamics(const S& s, const KukaParams& P, const float* qd, int u, unsigned gmask, KkPhaseClock* ph) {
 #else
 template <class S>
 KC_F void kc_dynamics(const S& s, const KukaParams& P, const float* qd) {
+    KkPhaseClock* const ph = nullptr;
 #endif
     KC_RUN(kc_ph_vel_terms(s, qd, u));
+    KK_PH(ph, KK_PH_DYN_D1);
     KC_RUN(kc_ph_prefix2(s, KB_W, KB_VO, 0.f, u));
+    KK_PH(ph, KK_PH_DYN_D2);
     KC_RUN(kc_ph_acc_terms(s, qd, u));
+    KK_PH(ph, KK_PH_DYN_D3);
     KC_RUN(kc_ph_prefix2(s, KB_AW, KB_AV, -P.gz, u));      // gravity as a fictitious base acceleration
+    KK_PH(ph, KK_PH_DYN_D4);
     KC_RUN(kc_ph_wrench(s, P, u));
+    KK_PH(ph, KK_PH_DYN_D5);
     KC_RUN(kc_ph_subtree(s, u));
+    KK_PH(ph, KK_PH_DYN_D6);
     KC_RUN(kc_ph_mass(s, u));
 }

@@ -35,19 +35,7 @@
 #define KK_PROBE_D(d)
 #define KK_PROBE_SWEEP()
 #endif
-// Diagnostic build (scripts/build_variant.sh phases -DKK_PHASES, scripts/kuka_phase_timing.py): clock64() accumulators per phase of the
-// micro-step loop, in registers, stored per env slot at the end of the launch.  Separate from KK_TIMING, whose convergence probe adds
-// instructions to every sweep row.  KK_PH(clk, k) charges the cycles since the previous mark to phase k; without KK_PHASES it is empty.
-// The fast sweeps are charged to one of two phases, by the copy of the loop the warp ran (no lane watching a contact, or the watch copy);
-// `nwatch` counts the physics steps of the slot that ran the watch copy.
-enum { KK_PH_KIN = 0, KK_PH_IK, KK_PH_DYN, KK_PH_CHOL, KK_PH_SETUP, KK_PH_FAST_QUIET, KK_PH_FAST_WATCH, KK_PH_GENERAL, KK_PH_ENV, KK_NPH };
-#if defined(KK_PHASES) && defined(__CUDACC__)
-struct KkPhaseClock { long long last; long long acc[KK_NPH]; unsigned nwatch; };
-#define KK_PH(clk, k) do { if (clk) { const long long t_ = clock64(); (clk)->acc[k] += t_ - (clk)->last; (clk)->last = t_; } } while (0)
-#else
-struct KkPhaseClock { long long dummy; };
-#define KK_PH(clk, k) do { (void)(clk); } while (0)
-#endif
+// (the phase clock of the -DKK_PHASES diagnostic build, KK_PH, is in kuka_coop.cuh: the four-lanes-per-env phases are marked too)
 struct f3 { float x, y, z; };
 struct alignas(16) kk_f4 { float x, y, z, w; };   // one 128-bit load (host-compilable stand-in for float4)
 KK_DEV f3 mk3(float x, float y, float z) { f3 r; r.x = x; r.y = y; r.z = z; return r; }
@@ -304,7 +292,7 @@ KK_DEV void quat_from_matrix(const float* R, float* q) {
 // dtheta = (J^T J + lambda I)^-1 J^T e over the 7 arm joints.  The 7x7 normal equations are formed and
 // solved in float64: they square the Jacobian's condition number, which float32 cannot afford.
 // Fully unrolled: rolled loops over thread-local arrays (smaller code) were local-memory-latency bound, measured slower.
-KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float* q_ik) {
+KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, float* q_ik, KkPhaseClock* ph = nullptr) {
     constexpr int n = 7;
     float J[6][n];
 #pragma unroll
@@ -343,6 +331,7 @@ KK_DEV void kuka_ik(const KukaParams& P, const KukaEnv& e, const KukaKin& k, flo
         for (int r = 0; r < 6; ++r) s = fma((double)J[r][i], (double)err[r], s);
         b[i] = s;
     }
+    KK_PH(ph, KK_PH_IK_BUILD);
     // Cholesky A = L L^T (A is SPD thanks to the damping), forward/back substitution
 #pragma unroll
     for (int j = 0; j < n; ++j) {
@@ -545,15 +534,15 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
         }
 #pragma unroll
         for (int t = 0; t < 9; ++t) kk7.R6[t] = sc[6 * KC_BS + KB_R + t];
-        kuka_ik(P, e, kk7, q_ik);
-    } else kuka_ik(P, e, k, q_ik);
-    KK_PH(ph, KK_PH_IK);
+        kuka_ik(P, e, kk7, q_ik, ph);
+    } else kuka_ik(P, e, k, q_ik, ph);
+    KK_PH(ph, KK_PH_IK_SOLVE);
     // ---- dynamics ----
     float A[KK_NB][KK_NB], bias[KK_NB];
     if constexpr (COOP) {
 #if defined(__CUDACC__)
         __syncwarp(gmask);      // every lane has read link 6's rotation: the wrench phase reuses its storage
-        kc_dynamics(sc, P, e.qd, u, gmask);
+        kc_dynamics(sc, P, e.qd, u, gmask, ph);
 #endif
 #pragma unroll
         for (int i = 0; i < KK_NB; ++i) {
@@ -561,14 +550,14 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
 #pragma unroll
             for (int j = 0; j <= i; ++j) A[i][j] = sc[KC_OFF_MA + i * KC_MS + j];
         }
-        KK_PH(ph, KK_PH_DYN);
+        KK_PH(ph, KK_PH_DYN_D7);
         // Cholesky + M^-1 in registers, by every lane: dealt to the 4 lanes through shared memory it was three times slower (12 dependent
         // pivot steps of load -> rsqrt -> scale -> store -> barrier)
         kuka_spd_inverse(A);
         KK_PH(ph, KK_PH_CHOL);
     } else {
         kuka_dynamics(P, e, k, A, bias);
-        KK_PH(ph, KK_PH_DYN);
+        KK_PH(ph, KK_PH_DYN_D7);
         kuka_spd_inverse(A);
         KK_PH(ph, KK_PH_CHOL);
     }
@@ -632,6 +621,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
     // ---- contact rows: J, W = M^-1 J^T (unscaled A), 1/D, target; two friction rows each.  Stored for the scaled system:
     //      J'_j = J_j / sigma_j and W'_j = sigma_j W_j on the 12 arm DoF, target' = target - J . tgt.  One row = KK_ROWW words: J'[0..13],
     //      1/D, target', W'[16..29] -- 16-byte groups, so that a row is eight 128-bit loads from the scratch area (COOP) or local memory. ----
+    KK_PH(ph, KK_PH_SETUP);
     const int nc = COOP ? nc_coop : ct.n;
     alignas(16) float cR[COOP ? 1 : 3 * KK_MAXC][KK_ROWW];
     float c_lam[3 * KK_MAXC];
@@ -761,7 +751,7 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
 #endif
     bool resume_mid_sweep = false;  // the fast loop already ran the motor + button rows of sweep it0
     bool watching = false;          // the warp ran the watch copy of the fast loop (phase attribution only)
-    KK_PH(ph, KK_PH_SETUP);
+    KK_PH(ph, KK_PH_ROWS);
     if ((lim_lo_mask | lim_hi_mask) == 0u) {
         // FAST LOOP (no arm joint on a limit): straight-line sweep, registers only.  Contact rows of the manifold are
         // WATCHED: while every normal row is separating (lam = 0 and J v >= target) it and its friction rows are exact
@@ -964,5 +954,5 @@ KK_DEV void kuka_physics_step(const KukaParams& P, KukaEnv& e, const KukaKin& k,
     for (int i = 0; i < KK_NB; ++i) { e.qd[i] = v[i]; e.q[i] = fmaf(P.dt, v[i], e.q[i]); }
     e.qdb = v[KK_NB]; e.qb = fmaf(P.dt, v[KK_NB], e.qb);
     if (TWOB) { e.qdb2 = v[ND - 1]; e.qb2 = fmaf(P.dt, v[ND - 1], e.qb2); }
-    KK_PH(ph, KK_PH_SETUP);
+    KK_PH(ph, KK_PH_EULER);
 }

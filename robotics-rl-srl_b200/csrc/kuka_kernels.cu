@@ -227,7 +227,7 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
 #endif
 #ifdef KK_PHASES
     KkPhaseClock kk_ph_clk; KkPhaseClock* const ph = &kk_ph_clk; unsigned kk_nphys = 0u;
-    kk_ph_clk.last = clock64();
+    kk_ph_clk.last = (unsigned)clock();
 #pragma unroll
     for (int k2 = 0; k2 < KK_NPH; ++k2) kk_ph_clk.acc[k2] = 0;
     kk_ph_clk.nwatch = 0u;
@@ -375,15 +375,15 @@ __global__ void __launch_bounds__(128, 1) kuka_kernel(const __grid_constant__ Ku
             kin.qb = e.qb; kin.qb2 = e.qb2; kin.bbx = e.bbx; kin.bby = e.bby; kin.bbz = e.bbz; kin.bb2x = e.bb2x; kin.bb2y = e.bb2y;
             KK_PH(ph, KK_PH_ENV);
             __syncwarp(gmask);   // the group is done with the rows / matrices of the previous micro-step (the candidates reuse that storage)
-            const bool near = kc_kinematics<TWOB>(sc, kc_tab, P, kin, u, gmask);
+            const bool near = kc_kinematics<TWOB>(sc, kc_tab, P, kin, u, gmask, ph);
             e.grip[0] = sc[8 * KC_BS + KB_C]; e.grip[1] = sc[8 * KC_BS + KB_C + 1]; e.grip[2] = sc[8 * KC_BS + KB_C + 2];   // getLinkState(kuka, 8)[0]: COM of link 8
             e.eepos[0] = sc[6 * KC_BS + KB_P]; e.eepos[1] = sc[6 * KC_BS + KB_P + 1]; e.eepos[2] = sc[6 * KC_BS + KB_P + 2];
             const int fl = near ? (int)sc[KC_OFF_LINK + 6] : 0;
             e.cbutton = fl & 1; e.ctable = (fl >> 1) & 1;
             if (TWOB) { e.cany0 = (fl >> 2) & 1; e.cany1 = (fl >> 3) & 1; }
             nc_reg = near ? (int)sc[KC_OFF_LINK + 7] : 0;
-            KK_PH(ph, KK_PH_KIN);
-        } else { KK_PH(ph, KK_PH_ENV); kuka_fk<TWOB>(P, e, k, ct); KK_PH(ph, KK_PH_KIN); }
+            KK_PH(ph, KK_PH_KIN_COLLECT);
+        } else { KK_PH(ph, KK_PH_ENV); kuka_fk<TWOB>(P, e, k, ct); KK_PH(ph, KK_PH_KIN_COLLECT); }
         const int new_cb = e.cbutton, new_ct = e.ctable, new_a0 = TWOB ? e.cany0 : 0, new_a1 = TWOB ? e.cany1 : 0;
         if (pending) {
             // ---- _reward() (:428-463): manifold of the step that just ran, link states after it ----

@@ -16,10 +16,15 @@ from srl_sim._abi import load_cuda_library
 from srl_sim.backend import Backend
 from srl_sim.model import load_kuka_scene
 
-PHASES = ["kinematics + collision", "IK (float64 7x7)", "dynamics (CRBA + RNEA)", "Cholesky + M^-1", "v0 + row set-up + scaling + Euler",
+# KK_PH_* of kuka_coop.cuh, in order
+PHASES = ["kin: local rotations", "kin: transform chain", "kin: body + candidates", "kin: collect + link states",
+          "IK: J, error, J^T J, J^T e", "IK: 7x7 solve",
+          "dyn D1 velocity terms", "dyn D2 velocity prefix", "dyn D3 acceleration terms", "dyn D4 acceleration prefix", "dyn D5 wrenches",
+          "dyn D6 sub-tree sums", "dyn D7 mass rows (+ load M, bias)",
+          "Cholesky + M^-1", "v0 + motor / limit set-up", "contact rows + scaling", "Euler",
           "fast sweeps, quiet copy", "fast sweeps, watch copy", "general loop", "env logic / loads / stores"]
 NPH = len(PHASES)
-FAST_QUIET, FAST_WATCH = 5, 6
+FAST_QUIET, FAST_WATCH = PHASES.index("fast sweeps, quiet copy"), PHASES.index("fast sweeps, watch copy")
 
 
 def main():
@@ -73,11 +78,11 @@ def main():
     sl = np.mean(slowest, axis=0)
     print("KukaButtonGymEnv-v0, %d envs x T = %d, %d live slots, %d launches after 3 warm-ups: %s ms per launch (phase-clock build)"
           % (n, T, per_step[0].shape[0], args.launches, " ".join("%.3f" % x for x in ms)))
-    print("%-36s %14s %14s %16s" % ("phase", "median cyc/step", "max cyc/step", "slowest slot %"))
+    print("%-38s %14s %14s %16s" % ("phase", "median cyc/step", "max cyc/step", "slowest slot %"))
     for k in range(NPH):
-        print("%-36s %14.0f %14.0f %15.1f%%" % (PHASES[k], np.median(ps[:, k]), np.max(ps[:, k]), 100.0 * sl[k] / sl.sum()))
+        print("%-38s %14.0f %14.0f %15.1f%%" % (PHASES[k], np.median(ps[:, k]), np.max(ps[:, k]), 100.0 * sl[k] / sl.sum()))
     tot = ps.sum(axis=1)
-    print("%-36s %14.0f %14.0f %15.1f%%" % ("total", np.median(tot), np.max(tot), 100.0))
+    print("%-38s %14.0f %14.0f %15.1f%%" % ("total", np.median(tot), np.max(tot), 100.0))
     print("slowest slot: %.0f cycles per launch = %.3f ms at 1.98 GHz" % (sl.sum(), sl.sum() / 1.98e6))
     ws = np.concatenate(watch_share)
     print("physics steps that ran the watch copy: slowest slot %.1f%% (mean over launches), median slot %.1f%%, all slots %.1f%%"
