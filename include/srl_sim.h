@@ -213,6 +213,17 @@ typedef struct srl_camera {
 } srl_camera;
 int srl_sim_render(srl_sim* sim, const srl_camera* camera, int width, int height, uint8_t* rgb_out, void* stream);
 
+/* One camera per env: cameras[i] draws env i (host array of N srl_camera, like srl_sim_render's camera).  follow_robot != 0
+ * (MobileRobot kinds only): the x and y of each camera's target are offsets from that env's robot position at the time of the call,
+ * computed as float32(float64 robot position + float64(offset)); the target's z stays absolute.  This is the reference's fpv camera
+ * (mobile_robot_env.py:316-326) with target offset (-0.25, 0, 0.15).  Output layout and frame contents as srl_sim_render: env i's frame
+ * is the bytes srl_sim_render(cameras[i]) gives it (with follow_robot: the camera with the absolute target).  The robot positions are read
+ * on the device.  The handle keeps the cameras it built last and reuses them when a call passes the same array (bytes), size and
+ * follow_robot again, so a caller that renders through fixed cameras every step pays no per-call host set-up.  The CPU oracle library
+ * does not export this entry point; the tests' CPU checker (tests/host/render_cameras_ref.cpp) implements it over oracle handles. */
+int srl_sim_render_cameras(srl_sim* sim, const srl_camera* cameras, int follow_robot, int width, int height,
+                           uint8_t* rgb_out, void* stream);
+
 /* Debug / single-env accessors (host arrays, synchronising; not on the hot path).  Derived link-state fields
  * (SRL_F_ROBOT_POS, SRL_F_EE_POS) reflect the last step or reset; they are not recomputed by set_state. */
 int srl_sim_get_state(srl_sim* sim, int field, void* dst, size_t bytes);

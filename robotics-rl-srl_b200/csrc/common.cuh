@@ -45,6 +45,8 @@ struct KukaDev;   // kuka_state.cuh
 struct KukaNext;  // kuka_kernels.cu
 struct DistDev;   // distractor_kernels.cu
 struct SrlBodyLooks;  // render_core.h
+struct SrlCam;        // render_core.h
+struct SrlCamFollow;  // render_core.h
 
 #define SRL_HOST_MAX_CHUNKS 16
 
@@ -82,6 +84,14 @@ struct srl_sim {
     float* render_prims; // [N][SRL_MAX_PRIMS][16] scene primitives of the last srl_sim_render (allocated on first use)
     float* render_prep;  // same shape: their per-camera prepared forms (render_core.h SrlPrep)
     int* render_counts;
+    // srl_sim_render_cameras (allocated on first use): every env's camera, the follow_robot inputs, their pinned staging buffer and the event
+    // of its last upload, and the camera array, size and follow_robot of the last call (the cameras are rebuilt only when these change)
+    SrlCam* render_cams;          // [N]
+    SrlCamFollow* render_follow;  // [N]
+    void* render_cam_stage;
+    cudaEvent_t render_cam_ev;
+    srl_camera* render_cam_key;   // [N], host
+    int render_cam_follow, render_cam_w, render_cam_h, render_cam_valid;
 };
 
 static inline bool srl_is_mobile(int kind) { return kind >= SRL_ENV_MOBILE && kind <= SRL_ENV_MOBILE_LINE_TARGET; }
@@ -98,6 +108,7 @@ int mobile_set_state(srl_sim* s, int field, const void* src, size_t bytes);
 
 // ---- image observations (render_kernels.cu) ------------------------------------------------
 int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint8_t* rgb, cudaStream_t st);
+int render_cams_launch(srl_sim* s, const srl_camera* cams, int follow_robot, int width, int height, uint8_t* rgb, cudaStream_t st);
 void render_free(srl_sim* s);
 
 // ---- launchers (kuka_kernels.cu) ---------------------------------------------------------

@@ -75,33 +75,90 @@ SRL_RHD void srl_prim_plane(SrlPrim& p, float z, float checker, float r, float g
 
 // ---- camera: pybullet's computeViewMatrixFromYawPitchRoll (upAxisIndex = 2) + computeProjectionMatrixFOV, as eye + basis (RECALLED from
 //      PhysicsClientC_API.cpp: eye = target + Rz(yaw) Ry(roll) Rx(pitch) (0, -distance, 0), up = the same rotation of (0, 0, 1)) ----
-SRL_RHD void srl_camera_setup(const float* target, float distance, float yaw_deg, float pitch_deg, float roll_deg, float fov_deg, int W, int H, SrlCam& c) {
+// It is built in two parts.  The angle part (the trigonometry) runs on the host only.  The target part runs on the host, and on the device
+// for cameras whose target follows the robot (srl_sim_render_cameras): it is written in explicitly rounded operations -- no FMA contraction,
+// IEEE square root and division on both sides -- so that a camera finished on the device has the bits the host gives it.
+struct SrlCamAngles { float R[9], distance, ub, su, vb, sv; };   // R = Rz(yaw) Ry(roll) Rx(pitch); ub..sv as in SrlCam
+// a camera whose target is the robot's position plus off (x, y; z absolute), finished on the device
+struct SrlCamFollow { SrlCamAngles a; float off[3]; };
+
+SRL_RHD float srl_mul_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+SRL_RHD float srl_add_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+SRL_RHD float srl_sub_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+SRL_RHD float srl_div_rn(float a, float b) {
+#if defined(__CUDA_ARCH__)
+    return __fdiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+SRL_RHD float srl_sqrt_rn(float a) {
+#if defined(__CUDA_ARCH__)
+    return __fsqrt_rn(a);
+#else
+    return sqrtf(a);
+#endif
+}
+
+SRL_RHD void srl_camera_angles(float distance, float yaw_deg, float pitch_deg, float roll_deg, float fov_deg, int W, int H, SrlCamAngles& a) {
     const float d2r = 0.01745329251994329547f;
     const float cy = cosf(yaw_deg * d2r), sy = sinf(yaw_deg * d2r), cp = cosf(pitch_deg * d2r), sp = sinf(pitch_deg * d2r);
     const float cr = cosf(roll_deg * d2r), sr = sinf(roll_deg * d2r);
-    // R = Rz(yaw) Ry(roll) Rx(pitch)
     const float R[9] = {cy * cr, cy * sr * sp - sy * cp, cy * sr * cp + sy * sp,
                         sy * cr, sy * sr * sp + cy * cp, sy * sr * cp - cy * sp,
                         -sr, cr * sp, cr * cp};
-    const float e[3] = {0.f, -distance, 0.f};
+    for (int i = 0; i < 9; ++i) a.R[i] = R[i];
+    a.distance = distance;
+    const float th = tanf(0.5f * fov_deg * d2r), aspect = (float)W / (float)H;      // computeProjectionMatrixFOV: vertical fov, aspect = width / height
+    a.ub = -th * aspect; a.su = 2.f * th * aspect / (float)W;
+    a.vb = th; a.sv = 2.f * th / (float)H;
+}
+
+SRL_RHD void srl_camera_target(const float* target, const SrlCamAngles& a, SrlCam& c) {
+    const float* R = a.R;
+    const float e[3] = {0.f, -a.distance, 0.f};
     float up0[3], f[3];
     for (int i = 0; i < 3; ++i) {
-        c.eye[i] = target[i] + R[3 * i] * e[0] + R[3 * i + 1] * e[1] + R[3 * i + 2] * e[2];
+        c.eye[i] = srl_add_rn(srl_add_rn(srl_add_rn(target[i], srl_mul_rn(R[3 * i], e[0])), srl_mul_rn(R[3 * i + 1], e[1])), srl_mul_rn(R[3 * i + 2], e[2]));
         up0[i] = R[3 * i + 2];
-        f[i] = target[i] - c.eye[i];
+        f[i] = srl_sub_rn(target[i], c.eye[i]);
     }
-    const float fl = sqrtf(f[0] * f[0] + f[1] * f[1] + f[2] * f[2]);
-    for (int i = 0; i < 3; ++i) c.fwd[i] = f[i] / fl;
+    const float fl = srl_sqrt_rn(srl_add_rn(srl_add_rn(srl_mul_rn(f[0], f[0]), srl_mul_rn(f[1], f[1])), srl_mul_rn(f[2], f[2])));
+    for (int i = 0; i < 3; ++i) c.fwd[i] = srl_div_rn(f[i], fl);
     // right = fwd x up0, up = right x fwd (the lookAt basis of b3ComputeViewMatrixFromPositions)
-    float s[3] = {c.fwd[1] * up0[2] - c.fwd[2] * up0[1], c.fwd[2] * up0[0] - c.fwd[0] * up0[2], c.fwd[0] * up0[1] - c.fwd[1] * up0[0]};
-    const float sl = sqrtf(s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
-    for (int i = 0; i < 3; ++i) c.right[i] = s[i] / sl;
-    c.up[0] = c.right[1] * c.fwd[2] - c.right[2] * c.fwd[1];
-    c.up[1] = c.right[2] * c.fwd[0] - c.right[0] * c.fwd[2];
-    c.up[2] = c.right[0] * c.fwd[1] - c.right[1] * c.fwd[0];
-    const float th = tanf(0.5f * fov_deg * d2r), aspect = (float)W / (float)H;      // computeProjectionMatrixFOV: vertical fov, aspect = width / height
-    c.ub = -th * aspect; c.su = 2.f * th * aspect / (float)W;
-    c.vb = th; c.sv = 2.f * th / (float)H;
+    const float s[3] = {srl_sub_rn(srl_mul_rn(c.fwd[1], up0[2]), srl_mul_rn(c.fwd[2], up0[1])),
+                        srl_sub_rn(srl_mul_rn(c.fwd[2], up0[0]), srl_mul_rn(c.fwd[0], up0[2])),
+                        srl_sub_rn(srl_mul_rn(c.fwd[0], up0[1]), srl_mul_rn(c.fwd[1], up0[0]))};
+    const float sl = srl_sqrt_rn(srl_add_rn(srl_add_rn(srl_mul_rn(s[0], s[0]), srl_mul_rn(s[1], s[1])), srl_mul_rn(s[2], s[2])));
+    for (int i = 0; i < 3; ++i) c.right[i] = srl_div_rn(s[i], sl);
+    c.up[0] = srl_sub_rn(srl_mul_rn(c.right[1], c.fwd[2]), srl_mul_rn(c.right[2], c.fwd[1]));
+    c.up[1] = srl_sub_rn(srl_mul_rn(c.right[2], c.fwd[0]), srl_mul_rn(c.right[0], c.fwd[2]));
+    c.up[2] = srl_sub_rn(srl_mul_rn(c.right[0], c.fwd[1]), srl_mul_rn(c.right[1], c.fwd[0]));
+    c.ub = a.ub; c.su = a.su; c.vb = a.vb; c.sv = a.sv;
+}
+
+SRL_RHD void srl_camera_setup(const float* target, float distance, float yaw_deg, float pitch_deg, float roll_deg, float fov_deg, int W, int H, SrlCam& c) {
+    SrlCamAngles a;
+    srl_camera_angles(distance, yaw_deg, pitch_deg, roll_deg, fov_deg, W, H, a);
+    srl_camera_target(target, a, c);
 }
 
 // ---- rotation by a unit quaternion q = (x y z w) and by its inverse, v' = v + w t + u x t with u = (x y z), t = 2 u x v (for the inverse

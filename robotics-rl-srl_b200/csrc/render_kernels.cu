@@ -98,6 +98,33 @@ __global__ void prepare_kernel(const float* __restrict__ prims, const int* __res
     if (prim_rect(cam, p, r)) { q.u0 = r.u0; q.u1 = r.u1; q.v0 = r.v0; q.v1 = r.v1; }       // else: srl_prepare's "everywhere"
     reinterpret_cast<SrlPrep*>(prep)[i] = q;
 }
+// the same with one camera per env (srl_sim_render_cameras): the thread takes cams[env]
+__global__ void prepare_cams_kernel(const float* __restrict__ prims, const int* __restrict__ counts, const SrlCam* __restrict__ cams, int n,
+                                    float* __restrict__ prep) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int env = i / SRL_MAX_PRIMS, k = i % SRL_MAX_PRIMS;
+    if (env >= n || k >= counts[env]) return;
+    const SrlCam cam = cams[env];
+    const SrlPrim p = reinterpret_cast<const SrlPrim*>(prims)[i];
+    SrlPrep q;
+    srl_prepare(cam.eye, p, q);
+    ScreenRect r;
+    if (prim_rect(cam, p, r)) { q.u0 = r.u0; q.u1 = r.u1; q.v0 = r.v0; q.v1 = r.v1; }
+    reinterpret_cast<SrlPrep*>(prep)[i] = q;
+}
+
+// follow_robot: one thread per env finishes its camera from the robot's position, as the host would for the target
+// float32(float64 position + float64 offset) (srl_camera_target gives the host's bits)
+__global__ void follow_cams_kernel(const SrlCamFollow* __restrict__ in, const double2* __restrict__ pos, int n, SrlCam* __restrict__ cams) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const SrlCamFollow f = in[i];
+    const double2 p = pos[i];
+    const float target[3] = {(float)(p.x + (double)f.off[0]), (float)(p.y + (double)f.off[1]), f.off[2]};
+    SrlCam c;
+    srl_camera_target(target, f.a, c);
+    cams[i] = c;
+}
 
 // One CTA = one 32 x 16 pixel tile of one env's frame, one warp = an 8 x 8 pixel block of it (two pixels per thread, four rows apart).  Each
 // warp first tests, one lane per primitive, whether the primitive's screen-space bound overlaps its block (conservative: a dropped primitive
@@ -107,9 +134,11 @@ __global__ void prepare_kernel(const float* __restrict__ prims, const int* __res
 #define SRL_TILE_W 32
 #define SRL_TILE_H 16
 // BODIES: the lists may hold oriented boxes (a Kuka handle with distractor bodies); the kernel for the other lists leaves their code out.
+// The body is shared by raster_kernel (one camera, a kernel parameter) and raster_cams_kernel (one camera per env, staged in shared memory
+// before the __syncthreads below).
 template <bool CULL, bool BODIES>
-__global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, SrlCam cam,
-                                                      int W, int H, uint8_t* __restrict__ rgb) {
+__device__ __forceinline__ void raster_tile(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, const SrlCam& cam,
+                                            int W, int H, uint8_t* __restrict__ rgb) {
     static_assert(SRL_MAX_PRIMS <= 64, "the kept set is a 64-bit mask");
     __shared__ __align__(16) SrlPrep sq[SRL_MAX_PRIMS];
     __shared__ __align__(16) uint8_t tile[SRL_TILE_H][3 * SRL_TILE_W];
@@ -163,10 +192,50 @@ __global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ p
         o[w] = reinterpret_cast<const uint32_t*>(tile[row])[w];
     }
 }
+template <bool CULL, bool BODIES>
+__global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, SrlCam cam,
+                                                      int W, int H, uint8_t* __restrict__ rgb) {
+    raster_tile<CULL, BODIES>(prims, prep, counts, cam, W, H, rgb);
+}
+// one camera per env: the CTA loads cams[env] (64 bytes) into shared memory once, for the culling test and the pixel rays
+template <bool CULL, bool BODIES>
+__global__ void __launch_bounds__(256) raster_cams_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts,
+                                                           const SrlCam* __restrict__ cams, int W, int H, uint8_t* __restrict__ rgb) {
+    static_assert(sizeof(SrlCam) % 16 == 0, "the camera is staged as float4 words");
+    __shared__ __align__(16) SrlCam scam;
+    if (threadIdx.x < sizeof(SrlCam) / 16) reinterpret_cast<float4*>(&scam)[threadIdx.x] = reinterpret_cast<const float4*>(cams + blockIdx.z)[threadIdx.x];
+    raster_tile<CULL, BODIES>(prims, prep, counts, scam, W, H, rgb);
+}
 
-}  // namespace
+// every env's frame from the prepared lists: through one camera (cam) or through cams[env] (cams != nullptr, device memory)
+template <bool CULL, bool BODIES>
+void raster_launch(dim3 grid, const float* pr, const float* pp, const int* cn, const SrlCam& cam, const SrlCam* cams, int W, int H, uint8_t* out, cudaStream_t st) {
+    if (cams) raster_cams_kernel<CULL, BODIES><<<grid, 256, 0, st>>>(pr, pp, cn, cams, W, H, out);
+    else raster_kernel<CULL, BODIES><<<grid, 256, 0, st>>>(pr, pp, cn, cam, W, H, out);
+}
+int raster_frames(srl_sim* s, const SrlCam& cam, const SrlCam* cams, int width, int height, uint8_t* rgb, cudaStream_t st) {
+    const bool no_cull = getenv("SRL_RENDER_NO_CULL") != nullptr;       // debugging aid: the block test is conservative, so both paths give the same bytes (tests/test_render_gpu.py)
+    const size_t per_env = (size_t)SRL_MAX_PRIMS * SRL_PRIM_WORDS;
+    const bool bodies = s->dist != nullptr;
+    for (int e0 = 0; e0 < s->n; e0 += 65535) {                           // grid.z is limited to 65535
+        const dim3 grid((width + SRL_TILE_W - 1) / SRL_TILE_W, (height + SRL_TILE_H - 1) / SRL_TILE_H, min(65535, s->n - e0));
+        uint8_t* out = rgb + (size_t)e0 * height * width * 3;
+        const float* pr = s->render_prims + e0 * per_env; const float* pp = s->render_prep + e0 * per_env; const int* cn = s->render_counts + e0;
+        const SrlCam* cm = cams ? cams + e0 : nullptr;
+        if (bodies) {
+            if (no_cull) raster_launch<false, true>(grid, pr, pp, cn, cam, cm, width, height, out, st);
+            else raster_launch<true, true>(grid, pr, pp, cn, cam, cm, width, height, out, st);
+        } else {
+            if (no_cull) raster_launch<false, false>(grid, pr, pp, cn, cam, cm, width, height, out, st);
+            else raster_launch<true, false>(grid, pr, pp, cn, cam, cm, width, height, out, st);
+        }
+    }
+    SRL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
 
-int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint8_t* rgb, cudaStream_t st) {
+// every env's primitive list from its state, into the buffers allocated on first use
+int render_lists(srl_sim* s, cudaStream_t st) {
     if (!s->render_prims) {
         SRL_CUDA_OK(cudaMalloc(&s->render_prims, (size_t)s->n * SRL_MAX_PRIMS * SRL_PRIM_WORDS * sizeof(float)));
         SRL_CUDA_OK(cudaMalloc(&s->render_prep, (size_t)s->n * SRL_MAX_PRIMS * SRL_PRIM_WORDS * sizeof(float)));
@@ -175,26 +244,71 @@ int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint
     if (srl_is_mobile(s->kind)) {
         mobile_prims_kernel<<<(s->n + 127) / 128, 128, 0, st>>>(s->mob, s->n, s->kind, s->render_prims, s->render_counts);
         SRL_CUDA_OK(cudaGetLastError());
-    } else if (kuka_render_prims(s, s->render_prims, s->render_counts, st)) return 1;
+        return 0;
+    }
+    return kuka_render_prims(s, s->render_prims, s->render_counts, st);
+}
+
+}  // namespace
+
+int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint8_t* rgb, cudaStream_t st) {
+    if (render_lists(s, st)) return 1;
     SrlCam c;
     srl_camera_setup(cam->target, cam->distance, cam->yaw, cam->pitch, cam->roll, cam->fov, width, height, c);
     prepare_kernel<<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, c, s->n, s->render_prep);
-    const bool no_cull = getenv("SRL_RENDER_NO_CULL") != nullptr;       // debugging aid: the block test is conservative, so both paths give the same bytes (tests/test_render_gpu.py)
-    const size_t per_env = (size_t)SRL_MAX_PRIMS * SRL_PRIM_WORDS;
-    const bool bodies = s->dist != nullptr;
-    for (int e0 = 0; e0 < s->n; e0 += 65535) {                           // grid.z is limited to 65535
-        const dim3 grid((width + SRL_TILE_W - 1) / SRL_TILE_W, (height + SRL_TILE_H - 1) / SRL_TILE_H, min(65535, s->n - e0));
-        uint8_t* out = rgb + (size_t)e0 * height * width * 3;
-        const float* pr = s->render_prims + e0 * per_env; const float* pp = s->render_prep + e0 * per_env; const int* cn = s->render_counts + e0;
-        if (bodies) {
-            if (no_cull) raster_kernel<false, true><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
-            else raster_kernel<true, true><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
-        } else {
-            if (no_cull) raster_kernel<false, false><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
-            else raster_kernel<true, false><<<grid, 256, 0, st>>>(pr, pp, cn, c, width, height, out);
-        }
+    if (raster_frames(s, c, nullptr, width, height, rgb, st)) return 1;
+    s->launches += 3;
+    return 0;
+}
+
+// One camera per env.  The host builds the cameras (every env's SrlCam, or with follow_robot its angle part and target offset) into a pinned
+// staging buffer and uploads them on the stream; the handle keeps the last camera array it built (with the size and follow_robot) and skips
+// both when a call passes the same bytes again, so a loop that renders through the same cameras every step does no host work per call.
+int render_cams_launch(srl_sim* s, const srl_camera* cams, int follow_robot, int width, int height, uint8_t* rgb, cudaStream_t st) {
+    if (render_lists(s, st)) return 1;
+    const size_t n = (size_t)s->n;
+    if (!s->render_cam_key) {       // allocated last: a call after a failed allocation retries the missing buffers
+        if (!s->render_cams) SRL_CUDA_OK(cudaMalloc(&s->render_cams, n * sizeof(SrlCam)));
+        if (!s->render_follow) SRL_CUDA_OK(cudaMalloc(&s->render_follow, n * sizeof(SrlCamFollow)));
+        if (!s->render_cam_stage)
+            SRL_CUDA_OK(cudaMallocHost(&s->render_cam_stage, n * (sizeof(SrlCamFollow) > sizeof(SrlCam) ? sizeof(SrlCamFollow) : sizeof(SrlCam))));
+        if (!s->render_cam_ev) SRL_CUDA_OK(cudaEventCreateWithFlags(&s->render_cam_ev, cudaEventDisableTiming));
+        s->render_cam_key = (srl_camera*)malloc(n * sizeof(srl_camera));
+        if (!s->render_cam_key) { srl_set_error("render_cameras: out of memory"); return 1; }
+        s->render_cam_valid = 0;
     }
-    SRL_CUDA_OK(cudaGetLastError());
+    const bool same = s->render_cam_valid && s->render_cam_follow == follow_robot && s->render_cam_w == width && s->render_cam_h == height &&
+                      memcmp(s->render_cam_key, cams, n * sizeof(srl_camera)) == 0;
+    if (!same) {
+        s->render_cam_valid = 0;
+        SRL_CUDA_OK(cudaEventSynchronize(s->render_cam_ev));            // the previous upload has left the staging buffer
+        if (follow_robot) {
+            SrlCamFollow* f = reinterpret_cast<SrlCamFollow*>(s->render_cam_stage);
+            for (size_t i = 0; i < n; ++i) {
+                const srl_camera& c = cams[i];
+                srl_camera_angles(c.distance, c.yaw, c.pitch, c.roll, c.fov, width, height, f[i].a);
+                for (int k = 0; k < 3; ++k) f[i].off[k] = c.target[k];
+            }
+            SRL_CUDA_OK(cudaMemcpyAsync(s->render_follow, f, n * sizeof(SrlCamFollow), cudaMemcpyHostToDevice, st));
+        } else {
+            SrlCam* o = reinterpret_cast<SrlCam*>(s->render_cam_stage);
+            for (size_t i = 0; i < n; ++i) {
+                const srl_camera& c = cams[i];
+                srl_camera_setup(c.target, c.distance, c.yaw, c.pitch, c.roll, c.fov, width, height, o[i]);
+            }
+            SRL_CUDA_OK(cudaMemcpyAsync(s->render_cams, o, n * sizeof(SrlCam), cudaMemcpyHostToDevice, st));
+        }
+        SRL_CUDA_OK(cudaEventRecord(s->render_cam_ev, st));
+        memcpy(s->render_cam_key, cams, n * sizeof(srl_camera));
+        s->render_cam_follow = follow_robot; s->render_cam_w = width; s->render_cam_h = height;
+        s->render_cam_valid = 1;
+    }
+    if (follow_robot) {     // the targets move with the robots: finish every camera from the current positions, on the device
+        follow_cams_kernel<<<(s->n + 127) / 128, 128, 0, st>>>(s->render_follow, s->mob.pos, s->n, s->render_cams);
+        s->launches += 1;
+    }
+    prepare_cams_kernel<<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, s->render_cams, s->n, s->render_prep);
+    if (raster_frames(s, SrlCam{}, s->render_cams, width, height, rgb, st)) return 1;
     s->launches += 3;
     return 0;
 }
@@ -203,5 +317,12 @@ void render_free(srl_sim* s) {
     if (s->render_prims) cudaFree(s->render_prims);
     if (s->render_prep) cudaFree(s->render_prep);
     if (s->render_counts) cudaFree(s->render_counts);
+    if (s->render_cams) cudaFree(s->render_cams);
+    if (s->render_follow) cudaFree(s->render_follow);
+    if (s->render_cam_stage) cudaFreeHost(s->render_cam_stage);
+    if (s->render_cam_ev) cudaEventDestroy(s->render_cam_ev);
+    free(s->render_cam_key);
     s->render_prims = nullptr; s->render_prep = nullptr; s->render_counts = nullptr;
+    s->render_cams = nullptr; s->render_follow = nullptr; s->render_cam_stage = nullptr; s->render_cam_ev = nullptr; s->render_cam_key = nullptr;
+    s->render_cam_valid = 0;
 }

@@ -262,6 +262,18 @@ int srl_sim_render(srl_sim* s, const srl_camera* camera, int width, int height, 
     return render_launch(s, camera, width, height, rgb_out, (cudaStream_t)stream);
 }
 
+int srl_sim_render_cameras(srl_sim* s, const srl_camera* cameras, int follow_robot, int width, int height, uint8_t* rgb_out, void* stream) {
+    if (!s || !cameras || !rgb_out) { srl_set_error("render_cameras: null argument"); return 1; }
+    if (width <= 0 || height <= 0 || width > 4096 || height > 4096) { srl_set_error("render_cameras: bad image size %d x %d", width, height); return 1; }
+    if (follow_robot && !srl_is_mobile(s->kind)) { srl_set_error("render_cameras: follow_robot needs a MobileRobot env kind (got kind %d)", s->kind); return 1; }
+    for (int i = 0; i < s->n; ++i) {
+        const srl_camera& c = cameras[i];
+        if (!(c.distance > 0.f) || !(c.fov > 0.f && c.fov < 180.f)) { srl_set_error("render_cameras: bad camera %d (distance %g, fov %g)", i, c.distance, c.fov); return 1; }
+    }
+    DeviceGuard guard(s->device);
+    return render_cams_launch(s, cameras, follow_robot, width, height, rgb_out, (cudaStream_t)stream);
+}
+
 int srl_sim_set_distractors(srl_sim* s, const void* assets_blob, size_t bytes) {
     if (!s) { srl_set_error("set_distractors: null handle"); return 1; }
     if (!srl_is_kuka(s->kind)) { srl_set_error("set_distractors: only KukaRandButtonGymEnv-v0 has distractor bodies"); return 1; }

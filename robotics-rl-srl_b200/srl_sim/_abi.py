@@ -93,12 +93,15 @@ _EXPORTS = [
     ("srl_sim_destroy", None, [c_void_p]),
 ]
 
-# opt-in features that only the CUDA library implements (the CPU oracle does not): bound when the library exports them
+# entry points the CUDA library implements and the CPU oracle library does not export itself (the tests' CPU checker of per-env cameras
+# adds srl_sim_render_cameras over it): bound when the library exports them
 _OPTIONAL_EXPORTS = [
     ("srl_sim_set_distractors", c_int, [c_void_p, c_void_p, c_size_t]),
+    ("srl_sim_render_cameras", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
 ]
 
-EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS + _OPTIONAL_EXPORTS]   # everything include/srl_sim.h declares
+OPTIONAL_SYMBOLS = [e[0] for e in _OPTIONAL_EXPORTS]
+EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS] + OPTIONAL_SYMBOLS   # everything include/srl_sim.h declares
 
 
 def _ptr(x):
@@ -245,6 +248,16 @@ class Sim(object):
         """One ``width`` x ``height`` RGB frame per env into ``rgb_out`` (u8[N, H, W, 3]); ``cam`` is an ``srl_sim.render.SrlCamera``."""
         rc = self._lib.srl_sim_render(self.handle, ctypes.byref(cam), int(width), int(height), _ptr(rgb_out), stream)
         self.library.check(rc, "srl_sim_render")
+
+    def render_cameras(self, cams, follow_robot, width, height, rgb_out, stream=None):
+        """One frame per env through its own camera: ``cams`` is a ctypes array of ``num_envs`` ``srl_sim.render.SrlCamera``; with
+        ``follow_robot`` (MobileRobot) each target's x and y are offsets from that env's robot position."""
+        if "srl_sim_render_cameras" not in self.library.optional:
+            raise SimError("%s does not implement per-env cameras" % self.library.path)
+        if cams is not None and len(cams) != self.num_envs:
+            raise ValueError("render_cameras: %d cameras for %d envs" % (len(cams), self.num_envs))
+        rc = self._lib.srl_sim_render_cameras(self.handle, cams, int(bool(follow_robot)), int(width), int(height), _ptr(rgb_out), stream)
+        self.library.check(rc, "srl_sim_render_cameras")
 
     def set_distractors(self, assets_blob):
         """KukaRandButtonGymEnv-v0 only, before the first reset: simulate the distractor bodies (``srl_sim.model.distractor_blob``).

@@ -40,6 +40,30 @@ def mobile_fpv_camera(robot_xy, yaw=90):
     return dict(target=(float(robot_xy[0]) - 0.25, float(robot_xy[1]), 0.15), distance=0.3, yaw=yaw, pitch=-17, roll=0, fov=90)
 
 
+# the first-person camera as offsets from the robot's position, for srl_sim_render_cameras(follow_robot=1): target (x - 0.25, y, 0.15)
+MOBILE_FPV_FOLLOW = mobile_fpv_camera((0.0, 0.0))
+
+
+def camera_array(cams):
+    """A ctypes array of ``SrlCamera``, one per env, from a list of camera dicts (build it once and reuse it: the library skips its
+    camera set-up when a call passes the same cameras as the previous one)."""
+    arr = (SrlCamera * len(cams))()
+    for i, c in enumerate(cams):
+        arr[i] = camera(**c)
+    return arr
+
+
+def render_cameras(sim, backend, cams, follow_robot=False, width=RENDER_WIDTH, height=RENDER_HEIGHT, out=None):
+    """One frame per env through its own camera: env ``i`` through ``cams[i]`` (a list of camera dicts or a ``camera_array``); with
+    ``follow_robot`` (MobileRobot) each target's x and y are offsets from that env's robot position, read on the device.
+    ``uint8 [N, H, W, 3]`` in the backend's memory."""
+    if not isinstance(cams, ctypes.Array):
+        cams = camera_array(cams)
+    buf = backend.zeros((sim.num_envs, height, width, 3), np.uint8) if out is None else out
+    sim.render_cameras(cams, follow_robot, width, height, buf, stream=backend.stream())
+    return buf
+
+
 def render_batch(sim, backend, cams, width=RENDER_WIDTH, height=RENDER_HEIGHT, out=None):
     """One frame per env and camera: ``uint8 [N, H, W, 3 * len(cams)]`` in the backend's memory (a CUDA tensor for the product library)."""
     n = sim.num_envs

@@ -51,6 +51,7 @@ class BatchedSRLVecEnv(object):
                                       % ("".join(" / " + m for m in kuka_state_models), srl_model))
         # raw_pixels: one rendered frame per env and camera (srl_sim/render.py; multi_view / fpv stack a second camera on the channels)
         self._cams = None
+        self._fpv_cams = None
         if srl_model == "raw_pixels":
             from . import render as _render
             if env_id.startswith("Kuka"):
@@ -58,7 +59,9 @@ class BatchedSRLVecEnv(object):
             else:
                 self._cams = [dict(_render.MOBILE_CAMERA, target=(2, 0, 0) if env_id == "MobileRobot1DGymEnv-v0" else (2, 2, 0))]
                 if env_kwargs.get("fpv", False):
-                    raise NotImplementedError("fpv frames follow each robot: use the single-env classes (one camera per env)")
+                    # each env's first-person camera follows its robot (mobile_robot_env.py:316-332): one camera per env, built once here
+                    # and finished from the robot positions on the device at every render
+                    self._fpv_cams = _render.camera_array([_render.MOBILE_FPV_FOLLOW] * int(num_envs))
         self.distractors = bool(env_kwargs.get("distractors", False))
         if self.distractors and env_id != "KukaRandButtonGymEnv-v0":
             raise ValueError("distractors=True is only available for KukaRandButtonGymEnv-v0 (got %r)" % env_id)
@@ -96,7 +99,8 @@ class BatchedSRLVecEnv(object):
             self._joints = np.tile(np.asarray(KUKA_INIT_JOINT_POSITIONS, np.float32), (self.num_envs, 1))
         if srl_model == "raw_pixels":
             from .render import RENDER_HEIGHT, RENDER_WIDTH
-            self.observation_space = spaces.Box(low=0, high=255, shape=(RENDER_HEIGHT, RENDER_WIDTH, 3 * len(self._cams)), dtype=np.uint8)
+            n_cams = len(self._cams) + (self._fpv_cams is not None)
+            self.observation_space = spaces.Box(low=0, high=255, shape=(RENDER_HEIGHT, RENDER_WIDTH, 3 * n_cams), dtype=np.uint8)
         else:
             out_dim = {"ground_truth": D, "joints": 14, "joints_position": D + 14}[srl_model]
             self.observation_space = spaces.Box(low=-np.inf, high=np.inf, shape=(out_dim,), dtype=np.float32)
@@ -122,10 +126,17 @@ class BatchedSRLVecEnv(object):
 
     # ---- VecEnv API (numpy) --------------------------------------------------------------------------
     def render_tensors(self):
-        """The current frame of every env, ``uint8 [N, H, W, 3 * cameras]`` in the backend's memory (a CUDA tensor on a GPU)."""
-        from .render import KUKA_CAMERA, MOBILE_CAMERA, render_batch
+        """The current frame of every env, ``uint8 [N, H, W, 3 * cameras]`` in the backend's memory (a CUDA tensor on a GPU); with ``fpv``
+        the first-person frames are the last three channels."""
+        from .render import KUKA_CAMERA, MOBILE_CAMERA, render_batch, render_cameras
         cams = self._cams or ([KUKA_CAMERA] if self.env_id.startswith("Kuka") else [MOBILE_CAMERA])
-        return render_batch(self.sim, self.backend, cams)
+        frames = render_batch(self.sim, self.backend, cams)
+        if self._fpv_cams is None:
+            return frames
+        fpv = render_cameras(self.sim, self.backend, self._fpv_cams, follow_robot=True)
+        if self.backend.on_gpu:
+            return self.backend.torch.cat([frames, fpv], dim=3)
+        return np.concatenate([frames, fpv], axis=3)
 
     def _state(self, obs):
         """ground-truth observation [N, D] -> the configured state (getSRLState), or the rendered frames (raw_pixels)."""
