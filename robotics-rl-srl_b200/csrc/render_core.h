@@ -180,7 +180,8 @@ SRL_RHD void srl_quat_rotate_inv(const float* q, const float* v, float* o) {
 //   PLANE   g0 = z - eye_z
 //   SPHERE  g0..2 = eye - centre, g3 = |eye - centre|^2 - r^2
 //   CAPSULE g0..2 = ba = end1 - end0, g3..5 = oa = eye - end0, g6 = ba.ba, g7 = ba.oa, g8 = ba.ba oa.oa - (ba.oa)^2 - r^2 ba.ba,
-//           g9 = oa.oa - r^2, g10 = |eye - end1|^2 - r^2                (a zero-length capsule is prepared as the SPHERE it is)
+//           g9 = oa.oa - r^2, g10 = |eye - end1|^2 - r^2                (a zero-length capsule is prepared as the SPHERE it is, and a
+//           capsule the eye is inside of as a sphere no ray reaches)
 //   CYL     g0, g1 = eye.xy - centre.xy, g2 = g0^2 + g1^2 - r^2, g3 = z0 - eye_z, g4 = z1 - eye_z, g5 = r^2
 //   BOX     g0..2 = eye - centre in the box frame, g3..5 = half extents, g6 = cos, g7 = sin
 //   OBOX    g0..2 = eye - centre in the box frame, g3..5 = half extents, g6..9 = the quaternion.  The ray is rotated into the box frame per
@@ -204,9 +205,13 @@ SRL_RHD void srl_prepare(const float* eye, const SrlPrim& p, SrlPrep& q) {
         const float ob[3] = {eye[0] - p.a[3], eye[1] - p.a[4], eye[2] - p.a[5]};
         const float baba = ba[0] * ba[0] + ba[1] * ba[1] + ba[2] * ba[2], baoa = ba[0] * oa[0] + ba[1] * oa[1] + ba[2] * oa[2];
         const float oaoa = oa[0] * oa[0] + oa[1] * oa[1] + oa[2] * oa[2];
-        if (baba < 1e-12f) {
+        const float k = baba < 1e-12f || baoa <= 0.f ? 0.f : baoa >= baba ? 1.f : baoa / baba;
+        const float w[3] = {oa[0] - k * ba[0], oa[1] - k * ba[1], oa[2] - k * ba[2]};
+        if (baba < 1e-12f || w[0] * w[0] + w[1] * w[1] + w[2] * w[2] < r * r) {
+            // an eye inside the capsule sees no entry point (a solid seen from inside is not drawn, as for the other types; the end sphere
+            // the ray leaves through is not its boundary there): prepared as a sphere no ray reaches
             q.type = (float)SRL_PRIM_SPHERE;
-            q.g[0] = oa[0]; q.g[1] = oa[1]; q.g[2] = oa[2]; q.g[3] = oaoa - r * r;
+            q.g[0] = oa[0]; q.g[1] = oa[1]; q.g[2] = oa[2]; q.g[3] = baba < 1e-12f ? oaoa - r * r : 1e30f;
         } else {
             for (int i = 0; i < 3; ++i) { q.g[i] = ba[i]; q.g[3 + i] = oa[i]; }
             q.g[6] = baba; q.g[7] = baoa; q.g[8] = baba * oaoa - baoa * baoa - r * r * baba;

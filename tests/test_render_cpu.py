@@ -17,6 +17,7 @@ import numpy as np
 import pytest
 
 from environments.registry import registered_env
+from render_numpy_ref import pybullet_matrices as _pybullet_matrices
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -82,27 +83,6 @@ def test_mobile_frame_layout_matches_the_reference_frame(use_oracle_backend):
     assert _line(ours["red"], 1) < 0.2 < 0.8 < _line(ours["green"], 1) and _line(ours["blue"], 0) < 0.2 < 0.8 < _line(ours["black"], 0)
     assert np.abs(_blob(ours["yellow"])[2:] - _blob(ref["yellow"])[2:]).max() < 0.012      # the disc of urdf/cylinder.urdf: same diameter
     env.close()
-
-
-def _pybullet_matrices(target, distance, yaw, pitch, roll, fov, aspect, near=0.1, far=100.0):
-    """numpy restatement of computeViewMatrixFromYawPitchRoll (upAxisIndex = 2) and computeProjectionMatrixFOV as MATRICES (the renderer uses
-    an eye + basis formulation): eye = target + Rz(yaw) Ry(roll) Rx(pitch) (0, -d, 0), up = the same rotation of (0, 0, 1), OpenGL lookAt and
-    perspective."""
-    y, p, r = np.radians([yaw, pitch, roll])
-    Rz = np.array([[np.cos(y), -np.sin(y), 0], [np.sin(y), np.cos(y), 0], [0, 0, 1]])
-    Ry = np.array([[np.cos(r), 0, np.sin(r)], [0, 1, 0], [-np.sin(r), 0, np.cos(r)]])
-    Rx = np.array([[1, 0, 0], [0, np.cos(p), -np.sin(p)], [0, np.sin(p), np.cos(p)]])
-    R = Rz @ Ry @ Rx
-    eye = np.asarray(target, float) + R @ np.array([0.0, -distance, 0.0])
-    up = R @ np.array([0.0, 0.0, 1.0])
-    f = np.asarray(target, float) - eye; f /= np.linalg.norm(f)
-    s = np.cross(f, up); s /= np.linalg.norm(s)
-    u = np.cross(s, f)
-    view = np.eye(4); view[0, :3], view[1, :3], view[2, :3] = s, u, -f
-    view[:3, 3] = -view[:3, :3] @ eye
-    t = 1.0 / np.tan(np.radians(fov) / 2)
-    proj = np.array([[t / aspect, 0, 0, 0], [0, t, 0, 0], [0, 0, (far + near) / (near - far), 2 * far * near / (near - far)], [0, 0, -1, 0]])
-    return view, proj
 
 
 def _project(point, view, proj, W, H):
