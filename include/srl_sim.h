@@ -197,7 +197,8 @@ int srl_sim_prefetch_resets(srl_sim* sim, void* stream);
  * distractor_blob; layout in csrc/distractor_core.h).  Valid only between srl_sim_create and the first reset, and not together with
  * srl_cfg.prefetch_resets.  With the bodies on, `reset_draws` rows are 48 wide: the 18 Kuka values, the 10 placements (x, y) as
  * final positions and the 10 object types (0-2); NULL = all from the env's counter-based stream.  The object types and the kick
- * direction come from the env's stream too (the reference draws them from the global, unseeded np.random).  State: SRL_F_DISTRACTORS. */
+ * direction come from the env's stream too (the reference draws them from the global, unseeded np.random).  State: SRL_F_DISTRACTORS.
+ * The CPU oracle library has no body dynamics: it exports this entry point and always returns 1. */
 int srl_sim_set_distractors(srl_sim* sim, const void* assets_blob, size_t bytes);
 
 /* Image observations (`srl_model = "raw_pixels"`): what the reference obtains per env from PyBullet's TinyRenderer in render(mode='rgb_array')
@@ -220,7 +221,7 @@ int srl_sim_render(srl_sim* sim, const srl_camera* camera, int width, int height
  * is the bytes srl_sim_render(cameras[i]) gives it (with follow_robot: the camera with the absolute target).  The robot positions are read
  * on the device.  The handle keeps the cameras it built last and reuses them when a call passes the same array (bytes), size and
  * follow_robot again, so a caller that renders through fixed cameras every step pays no per-call host set-up.  The CPU oracle library
- * does not export this entry point; the tests' CPU checker (tests/host/render_cameras_ref.cpp) implements it over oracle handles. */
+ * implements it too, on host arrays. */
 int srl_sim_render_cameras(srl_sim* sim, const srl_camera* cameras, int follow_robot, int width, int height,
                            uint8_t* rgb_out, void* stream);
 

@@ -9,7 +9,6 @@
 #include <string.h>
 #include <new>
 #include "oracle_sim.h"
-#include "../robotics-rl-srl_b200/csrc/render_core.h"
 
 static thread_local char g_err[512] = "";
 
@@ -213,30 +212,6 @@ static int mobile_set_state(srl_sim* s, int field, const void* src, size_t bytes
         oracle_set_error("set_state: field %d not settable for MobileRobot", field);
         return 1;
     }
-}
-
-/* CPU checker of the image path: the same primitive lists and per-pixel arithmetic (csrc/render_core.h), frames in host memory */
-int srl_sim_render(srl_sim* s, const srl_camera* cam, int width, int height, uint8_t* rgb_out, void*) {
-    if (!s || !cam || !rgb_out) { oracle_set_error("render: null argument"); return 1; }
-    if (width <= 0 || height <= 0) { oracle_set_error("render: bad image size"); return 1; }
-    SrlCam c;
-    srl_camera_setup(cam->target, cam->distance, cam->yaw, cam->pitch, cam->roll, cam->fov, width, height, c);
-    std::vector<SrlPrim> prims(SRL_MAX_PRIMS);
-    std::vector<SrlPrep> prep(SRL_MAX_PRIMS);
-    for (int i = 0; i < s->n; ++i) {
-        int np;
-        if (is_mobile(s->kind)) {
-            const MobileEnv& e = s->mobile[i];
-            const int rk = s->kind == SRL_ENV_MOBILE_2TARGET ? 1 : s->kind == SRL_ENV_MOBILE_LINE_TARGET ? 2 : s->kind == SRL_ENV_MOBILE_1D ? 3 : 0;
-            np = srl_mobile_scene(rk, (float)e.pos[0], (float)e.pos[1], (float)e.target[0][0], (float)e.target[0][1], (float)e.target[1][0], (float)e.target[1][1], prims.data());
-        } else np = oracle_kuka_scene(s, i, prims.data());
-        for (int k = 0; k < np; ++k) srl_prepare(c.eye, prims[k], prep[k]);
-        uint8_t* frame = rgb_out + (size_t)i * height * width * 3;
-        for (int y = 0; y < height; ++y)
-            for (int x = 0; x < width; ++x)
-                srl_render_pixel(c, prep.data(), prims.data(), srl_prim_mask_all(np), x, y, frame + ((size_t)y * width + x) * 3);
-    }
-    return 0;
 }
 
 int srl_sim_get_state(srl_sim* s, int field, void* dst, size_t bytes) {

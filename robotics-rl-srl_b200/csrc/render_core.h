@@ -13,6 +13,8 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
+#include "../../include/srl_sim.h"
 #include "distractor_core.h"
 
 #if defined(__CUDACC__)
@@ -159,6 +161,26 @@ SRL_RHD void srl_camera_setup(const float* target, float distance, float yaw_deg
     SrlCamAngles a;
     srl_camera_angles(distance, yaw_deg, pitch_deg, roll_deg, fov_deg, W, H, a);
     srl_camera_target(target, a, c);
+}
+
+// The argument checks of srl_sim_render (per_env false, one camera) and srl_sim_render_cameras (per_env true, n cameras), the same in both
+// libraries: nullptr, or the message, written into msg.
+inline const char* srl_render_args_error(bool per_env, int env_kind, const srl_camera* cams, int n, int follow_robot, int W, int H, char* msg,
+                                         size_t len) {
+    const char* what = per_env ? "render_cameras" : "render";
+    if (W <= 0 || H <= 0 || W > 4096 || H > 4096) { snprintf(msg, len, "%s: bad image size %d x %d", what, W, H); return msg; }
+    if (follow_robot && !(env_kind >= SRL_ENV_MOBILE && env_kind <= SRL_ENV_MOBILE_LINE_TARGET)) {
+        snprintf(msg, len, "%s: follow_robot needs a MobileRobot env kind (got kind %d)", what, env_kind);
+        return msg;
+    }
+    for (int i = 0; i < n; ++i) {
+        const srl_camera& c = cams[i];
+        if (c.distance > 0.f && c.fov > 0.f && c.fov < 180.f) continue;
+        if (per_env) snprintf(msg, len, "%s: bad camera %d (distance %g, fov %g)", what, i, c.distance, c.fov);
+        else snprintf(msg, len, "%s: bad camera (distance %g, fov %g)", what, c.distance, c.fov);
+        return msg;
+    }
+    return nullptr;
 }
 
 // ---- rotation by a unit quaternion q = (x y z w) and by its inverse, v' = v + w t + u x t with u = (x y z), t = 2 u x v (for the inverse
@@ -455,7 +477,11 @@ SRL_RHD int srl_distractor_prims(const SrlBodyLooks& L, const float* B, int n, S
 
 // MobileRobot family: plane, four walls (urdf/wall.urdf: box 4 x 0.1 x 0.1; left red, bottom black, right green, top blue:
 // mobile_robot_env.py:184-203), the robot as a box of the racecar's footprint, the target(s).
-// kind: 0 base, 3 one-dimensional, 1 two targets, 2 line target (urdf/wall_target.urdf: box 4 x 0.5 x 0.1, yellow, rotated by pi / 2).
+// kind: 0 base, 3 one-dimensional, 1 two targets, 2 line target (urdf/wall_target.urdf: box 4 x 0.5 x 0.1, yellow, rotated by pi / 2),
+// from the env kind by srl_mobile_render_kind.
+SRL_RHD int srl_mobile_render_kind(int env_kind) {
+    return env_kind == SRL_ENV_MOBILE_2TARGET ? 1 : env_kind == SRL_ENV_MOBILE_LINE_TARGET ? 2 : env_kind == SRL_ENV_MOBILE_1D ? 3 : 0;
+}
 SRL_RHD int srl_mobile_scene(int kind, float rx, float ry, float t0x, float t0y, float t1x, float t1y, SrlPrim* out) {
     int n = 0;
     srl_prim_plane(out[n++], 0.f, 1.0f, 1.0f, 1.0f, 1.0f);

@@ -14,7 +14,7 @@ __global__ void mobile_prims_kernel(MobileDev d, int n, int kind, float* __restr
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const double2 pos = d.pos[i], t0 = d.tgt0[i], t1 = d.tgt1[i];
-    const int rk = kind == SRL_ENV_MOBILE_2TARGET ? 1 : kind == SRL_ENV_MOBILE_LINE_TARGET ? 2 : kind == SRL_ENV_MOBILE_1D ? 3 : 0;
+    const int rk = srl_mobile_render_kind(kind);
     SrlPrim* out = reinterpret_cast<SrlPrim*>(prims + (size_t)i * SRL_MAX_PRIMS * SRL_PRIM_WORDS);
     counts[i] = srl_mobile_scene(rk, (float)pos.x, (float)pos.y, (float)t0.x, (float)t0.y, (float)t1.x, (float)t1.y, out);
 }
@@ -86,30 +86,26 @@ __device__ __forceinline__ bool prim_rect(const SrlCam& c, const SrlPrim& p, Scr
     return false;
 }
 
+// The camera argument of the prepare and raster kernels: one SrlCam for the batch, a kernel parameter (srl_sim_render), or with PER_ENV
+// one per env in device memory (srl_sim_render_cameras).
+template <bool PER_ENV> struct CamArg { typedef SrlCam type; };
+template <> struct CamArg<true> { typedef const SrlCam* __restrict__ type; };
+__device__ __forceinline__ const SrlCam& env_cam(const SrlCam& cam, int) { return cam; }
+__device__ __forceinline__ SrlCam env_cam(const SrlCam* __restrict__ cams, int env) { return cams[env]; }
+
 // One thread per (env, primitive): the per-camera prepared form (render_core.h) plus the screen-space bound, [N][SRL_MAX_PRIMS][16 floats].
-__global__ void prepare_kernel(const float* __restrict__ prims, const int* __restrict__ counts, SrlCam cam, int n, float* __restrict__ prep) {
+template <bool PER_ENV>
+__global__ void prepare_kernel(const float* __restrict__ prims, const int* __restrict__ counts, typename CamArg<PER_ENV>::type cams, int n,
+                               float* __restrict__ prep) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int env = i / SRL_MAX_PRIMS, k = i % SRL_MAX_PRIMS;
     if (env >= n || k >= counts[env]) return;
+    const SrlCam& cam = env_cam(cams, env);
     const SrlPrim p = reinterpret_cast<const SrlPrim*>(prims)[i];
     SrlPrep q;
     srl_prepare(cam.eye, p, q);
     ScreenRect r;
     if (prim_rect(cam, p, r)) { q.u0 = r.u0; q.u1 = r.u1; q.v0 = r.v0; q.v1 = r.v1; }       // else: srl_prepare's "everywhere"
-    reinterpret_cast<SrlPrep*>(prep)[i] = q;
-}
-// the same with one camera per env (srl_sim_render_cameras): the thread takes cams[env]
-__global__ void prepare_cams_kernel(const float* __restrict__ prims, const int* __restrict__ counts, const SrlCam* __restrict__ cams, int n,
-                                    float* __restrict__ prep) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int env = i / SRL_MAX_PRIMS, k = i % SRL_MAX_PRIMS;
-    if (env >= n || k >= counts[env]) return;
-    const SrlCam cam = cams[env];
-    const SrlPrim p = reinterpret_cast<const SrlPrim*>(prims)[i];
-    SrlPrep q;
-    srl_prepare(cam.eye, p, q);
-    ScreenRect r;
-    if (prim_rect(cam, p, r)) { q.u0 = r.u0; q.u1 = r.u1; q.v0 = r.v0; q.v1 = r.v1; }
     reinterpret_cast<SrlPrep*>(prep)[i] = q;
 }
 
@@ -134,8 +130,7 @@ __global__ void follow_cams_kernel(const SrlCamFollow* __restrict__ in, const do
 #define SRL_TILE_W 32
 #define SRL_TILE_H 16
 // BODIES: the lists may hold oriented boxes (a Kuka handle with distractor bodies); the kernel for the other lists leaves their code out.
-// The body is shared by raster_kernel (one camera, a kernel parameter) and raster_cams_kernel (one camera per env, staged in shared memory
-// before the __syncthreads below).
+// raster_kernel<..., PER_ENV = true> stages its env's camera in shared memory before the __syncthreads below.
 template <bool CULL, bool BODIES>
 __device__ __forceinline__ void raster_tile(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, const SrlCam& cam,
                                             int W, int H, uint8_t* __restrict__ rgb) {
@@ -192,43 +187,34 @@ __device__ __forceinline__ void raster_tile(const float* __restrict__ prims, con
         o[w] = reinterpret_cast<const uint32_t*>(tile[row])[w];
     }
 }
-template <bool CULL, bool BODIES>
-__global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts, SrlCam cam,
-                                                      int W, int H, uint8_t* __restrict__ rgb) {
-    raster_tile<CULL, BODIES>(prims, prep, counts, cam, W, H, rgb);
-}
-// one camera per env: the CTA loads cams[env] (64 bytes) into shared memory once, for the culling test and the pixel rays
-template <bool CULL, bool BODIES>
-__global__ void __launch_bounds__(256) raster_cams_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts,
-                                                           const SrlCam* __restrict__ cams, int W, int H, uint8_t* __restrict__ rgb) {
-    static_assert(sizeof(SrlCam) % 16 == 0, "the camera is staged as float4 words");
-    __shared__ __align__(16) SrlCam scam;
-    if (threadIdx.x < sizeof(SrlCam) / 16) reinterpret_cast<float4*>(&scam)[threadIdx.x] = reinterpret_cast<const float4*>(cams + blockIdx.z)[threadIdx.x];
-    raster_tile<CULL, BODIES>(prims, prep, counts, scam, W, H, rgb);
+// PER_ENV: the CTA loads cams[env] (64 bytes) into shared memory once, for the culling test and the pixel rays
+template <bool CULL, bool BODIES, bool PER_ENV>
+__global__ void __launch_bounds__(256) raster_kernel(const float* __restrict__ prims, const float* __restrict__ prep, const int* __restrict__ counts,
+                                                      typename CamArg<PER_ENV>::type cams, int W, int H, uint8_t* __restrict__ rgb) {
+    if constexpr (PER_ENV) {
+        static_assert(sizeof(SrlCam) % 16 == 0, "the camera is staged as float4 words");
+        __shared__ __align__(16) SrlCam scam;
+        if (threadIdx.x < sizeof(SrlCam) / 16) reinterpret_cast<float4*>(&scam)[threadIdx.x] = reinterpret_cast<const float4*>(cams + blockIdx.z)[threadIdx.x];
+        raster_tile<CULL, BODIES>(prims, prep, counts, scam, W, H, rgb);
+    } else {
+        raster_tile<CULL, BODIES>(prims, prep, counts, cams, W, H, rgb);
+    }
 }
 
-// every env's frame from the prepared lists: through one camera (cam) or through cams[env] (cams != nullptr, device memory)
-template <bool CULL, bool BODIES>
-void raster_launch(dim3 grid, const float* pr, const float* pp, const int* cn, const SrlCam& cam, const SrlCam* cams, int W, int H, uint8_t* out, cudaStream_t st) {
-    if (cams) raster_cams_kernel<CULL, BODIES><<<grid, 256, 0, st>>>(pr, pp, cn, cams, W, H, out);
-    else raster_kernel<CULL, BODIES><<<grid, 256, 0, st>>>(pr, pp, cn, cam, W, H, out);
-}
-int raster_frames(srl_sim* s, const SrlCam& cam, const SrlCam* cams, int width, int height, uint8_t* rgb, cudaStream_t st) {
+// every env's frame from the prepared lists, through the camera argument of the prepare kernel
+template <bool PER_ENV>
+int raster_frames(srl_sim* s, typename CamArg<PER_ENV>::type cams, int width, int height, uint8_t* rgb, cudaStream_t st) {
     const bool no_cull = getenv("SRL_RENDER_NO_CULL") != nullptr;       // debugging aid: the block test is conservative, so both paths give the same bytes (tests/test_render_gpu.py)
     const size_t per_env = (size_t)SRL_MAX_PRIMS * SRL_PRIM_WORDS;
     const bool bodies = s->dist != nullptr;
+    const auto kernel = bodies ? (no_cull ? raster_kernel<false, true, PER_ENV> : raster_kernel<true, true, PER_ENV>)
+                               : (no_cull ? raster_kernel<false, false, PER_ENV> : raster_kernel<true, false, PER_ENV>);
     for (int e0 = 0; e0 < s->n; e0 += 65535) {                           // grid.z is limited to 65535
         const dim3 grid((width + SRL_TILE_W - 1) / SRL_TILE_W, (height + SRL_TILE_H - 1) / SRL_TILE_H, min(65535, s->n - e0));
         uint8_t* out = rgb + (size_t)e0 * height * width * 3;
         const float* pr = s->render_prims + e0 * per_env; const float* pp = s->render_prep + e0 * per_env; const int* cn = s->render_counts + e0;
-        const SrlCam* cm = cams ? cams + e0 : nullptr;
-        if (bodies) {
-            if (no_cull) raster_launch<false, true>(grid, pr, pp, cn, cam, cm, width, height, out, st);
-            else raster_launch<true, true>(grid, pr, pp, cn, cam, cm, width, height, out, st);
-        } else {
-            if (no_cull) raster_launch<false, false>(grid, pr, pp, cn, cam, cm, width, height, out, st);
-            else raster_launch<true, false>(grid, pr, pp, cn, cam, cm, width, height, out, st);
-        }
+        if constexpr (PER_ENV) kernel<<<grid, 256, 0, st>>>(pr, pp, cn, cams + e0, width, height, out);
+        else kernel<<<grid, 256, 0, st>>>(pr, pp, cn, cams, width, height, out);
     }
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
@@ -255,8 +241,8 @@ int render_launch(srl_sim* s, const srl_camera* cam, int width, int height, uint
     if (render_lists(s, st)) return 1;
     SrlCam c;
     srl_camera_setup(cam->target, cam->distance, cam->yaw, cam->pitch, cam->roll, cam->fov, width, height, c);
-    prepare_kernel<<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, c, s->n, s->render_prep);
-    if (raster_frames(s, c, nullptr, width, height, rgb, st)) return 1;
+    prepare_kernel<false><<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, c, s->n, s->render_prep);
+    if (raster_frames<false>(s, c, width, height, rgb, st)) return 1;
     s->launches += 3;
     return 0;
 }
@@ -307,8 +293,8 @@ int render_cams_launch(srl_sim* s, const srl_camera* cams, int follow_robot, int
         follow_cams_kernel<<<(s->n + 127) / 128, 128, 0, st>>>(s->render_follow, s->mob.pos, s->n, s->render_cams);
         s->launches += 1;
     }
-    prepare_cams_kernel<<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, s->render_cams, s->n, s->render_prep);
-    if (raster_frames(s, SrlCam{}, s->render_cams, width, height, rgb, st)) return 1;
+    prepare_kernel<true><<<(s->n * SRL_MAX_PRIMS + 255) / 256, 256, 0, st>>>(s->render_prims, s->render_counts, s->render_cams, s->n, s->render_prep);
+    if (raster_frames<true>(s, s->render_cams, width, height, rgb, st)) return 1;
     s->launches += 3;
     return 0;
 }

@@ -7,6 +7,7 @@
 #include <string.h>
 #include <new>
 #include "common.cuh"
+#include "render_core.h"
 
 static thread_local char g_err[512] = "";
 
@@ -256,20 +257,16 @@ int srl_sim_rollout_host(srl_sim* s, int T, const void* actions, const float* no
 
 int srl_sim_render(srl_sim* s, const srl_camera* camera, int width, int height, uint8_t* rgb_out, void* stream) {
     if (!s || !camera || !rgb_out) { srl_set_error("render: null argument"); return 1; }
-    if (width <= 0 || height <= 0 || width > 4096 || height > 4096) { srl_set_error("render: bad image size %d x %d", width, height); return 1; }
-    if (!(camera->distance > 0.f) || !(camera->fov > 0.f && camera->fov < 180.f)) { srl_set_error("render: bad camera (distance %g, fov %g)", camera->distance, camera->fov); return 1; }
+    char msg[256];
+    if (srl_render_args_error(false, s->kind, camera, 1, 0, width, height, msg, sizeof(msg))) { srl_set_error("%s", msg); return 1; }
     DeviceGuard guard(s->device);
     return render_launch(s, camera, width, height, rgb_out, (cudaStream_t)stream);
 }
 
 int srl_sim_render_cameras(srl_sim* s, const srl_camera* cameras, int follow_robot, int width, int height, uint8_t* rgb_out, void* stream) {
     if (!s || !cameras || !rgb_out) { srl_set_error("render_cameras: null argument"); return 1; }
-    if (width <= 0 || height <= 0 || width > 4096 || height > 4096) { srl_set_error("render_cameras: bad image size %d x %d", width, height); return 1; }
-    if (follow_robot && !srl_is_mobile(s->kind)) { srl_set_error("render_cameras: follow_robot needs a MobileRobot env kind (got kind %d)", s->kind); return 1; }
-    for (int i = 0; i < s->n; ++i) {
-        const srl_camera& c = cameras[i];
-        if (!(c.distance > 0.f) || !(c.fov > 0.f && c.fov < 180.f)) { srl_set_error("render_cameras: bad camera %d (distance %g, fov %g)", i, c.distance, c.fov); return 1; }
-    }
+    char msg[256];
+    if (srl_render_args_error(true, s->kind, cameras, s->n, follow_robot, width, height, msg, sizeof(msg))) { srl_set_error("%s", msg); return 1; }
     DeviceGuard guard(s->device);
     return render_cams_launch(s, cameras, follow_robot, width, height, rgb_out, (cudaStream_t)stream);
 }

@@ -82,6 +82,8 @@ _EXPORTS = [
     ("srl_sim_rollout_host", c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     ("srl_sim_prefetch_resets", c_int, [c_void_p, c_void_p]),
     ("srl_sim_render", c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    ("srl_sim_render_cameras", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    ("srl_sim_set_distractors", c_int, [c_void_p, c_void_p, c_size_t]),
     ("srl_sim_get_state", c_int, [c_void_p, c_int, c_void_p, c_size_t]),
     ("srl_sim_set_state", c_int, [c_void_p, c_int, c_void_p, c_size_t]),
     ("srl_sim_launch_count", c_uint64, [c_void_p]),
@@ -93,15 +95,7 @@ _EXPORTS = [
     ("srl_sim_destroy", None, [c_void_p]),
 ]
 
-# entry points the CUDA library implements and the CPU oracle library does not export itself (the tests' CPU checker of per-env cameras
-# adds srl_sim_render_cameras over it): bound when the library exports them
-_OPTIONAL_EXPORTS = [
-    ("srl_sim_set_distractors", c_int, [c_void_p, c_void_p, c_size_t]),
-    ("srl_sim_render_cameras", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
-]
-
-OPTIONAL_SYMBOLS = [e[0] for e in _OPTIONAL_EXPORTS]
-EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS] + OPTIONAL_SYMBOLS   # everything include/srl_sim.h declares
+EXPORTED_SYMBOLS = [e[0] for e in _EXPORTS]   # everything include/srl_sim.h declares
 
 
 def _ptr(x):
@@ -136,13 +130,6 @@ class SimLibrary(object):
                 raise SimError("%s does not export %s" % (self.path, name))
             fn.restype = restype
             fn.argtypes = argtypes
-        self.optional = set()
-        for name, restype, argtypes in _OPTIONAL_EXPORTS:
-            fn = getattr(self.lib, name, None)
-            if fn is not None:
-                fn.restype = restype
-                fn.argtypes = argtypes
-                self.optional.add(name)
         v = self.lib.srl_sim_abi_version()
         if v != ABI_VERSION:
             raise SimError("ABI version mismatch: library %d, binding %d" % (v, ABI_VERSION))
@@ -252,8 +239,6 @@ class Sim(object):
     def render_cameras(self, cams, follow_robot, width, height, rgb_out, stream=None):
         """One frame per env through its own camera: ``cams`` is a ctypes array of ``num_envs`` ``srl_sim.render.SrlCamera``; with
         ``follow_robot`` (MobileRobot) each target's x and y are offsets from that env's robot position."""
-        if "srl_sim_render_cameras" not in self.library.optional:
-            raise SimError("%s does not implement per-env cameras" % self.library.path)
         if cams is not None and len(cams) != self.num_envs:
             raise ValueError("render_cameras: %d cameras for %d envs" % (len(cams), self.num_envs))
         rc = self._lib.srl_sim_render_cameras(self.handle, cams, int(bool(follow_robot)), int(width), int(height), _ptr(rgb_out), stream)
@@ -262,8 +247,6 @@ class Sim(object):
     def set_distractors(self, assets_blob):
         """KukaRandButtonGymEnv-v0 only, before the first reset: simulate the distractor bodies (``srl_sim.model.distractor_blob``).
         Observations, rewards and done flags do not change; the bodies' state is ``get_state(F_DISTRACTORS)``."""
-        if "srl_sim_set_distractors" not in self.library.optional:
-            raise SimError("%s does not implement distractor bodies" % self.library.path)
         self._dist_blob = np.ascontiguousarray(assets_blob, dtype=np.float64)
         rc = self._lib.srl_sim_set_distractors(self.handle, self._dist_blob.ctypes.data, self._dist_blob.nbytes)
         self.library.check(rc, "srl_sim_set_distractors")

@@ -1,33 +1,26 @@
 """
-CPU checker of KukaRandButton frames with distractor bodies (test-only): tests/host/distractor_frames_ref.cpp compiled once per process into
-a temporary directory against oracle/liboracle_sim.so.  `render` draws an oracle handle's scene plus caller-given bodies (the
-SRL_F_DISTRACTORS layout, f64[N][11][9]) through the same list builder and per-pixel arithmetic as the CUDA library.
+CPU checker of KukaRandButton frames with distractor bodies (test-only): `oracle_render_bodies` of oracle/liboracle_sim.so.  `render` draws
+an oracle handle's scene plus caller-given bodies (the SRL_F_DISTRACTORS layout, f64[N][11][9]) through the same list builder and per-pixel
+arithmetic as the CUDA library.
 """
 import ctypes
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ORACLE_DIR = os.path.join(ROOT, "oracle")
+ORACLE_LIB = os.path.join(ROOT, "oracle", "liboracle_sim.so")
 _lib = None
 
 
 def library():
     global _lib
     if _lib is None:
-        subprocess.check_call(["make", "-s", "-C", ORACLE_DIR])
-        out = os.path.join(tempfile.mkdtemp(prefix="dfr_"), "libdistractor_frames_ref.so")
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-Wall", "-shared", "-o", out,
-                               os.path.join(ROOT, "tests", "host", "distractor_frames_ref.cpp"), os.path.join(ORACLE_DIR, "liboracle_sim.so"),
-                               "-Wl,-rpath," + ORACLE_DIR])
-        lib = ctypes.CDLL(out)
+        from srl_sim._abi import SimLibrary
+        lib = SimLibrary(ORACLE_LIB).lib
         P = ctypes.c_void_p
-        lib.dfr_render.restype = ctypes.c_int
-        lib.dfr_render.argtypes = [P, P, ctypes.c_size_t, P, P, ctypes.c_int, ctypes.c_int, P]
-        lib.dfr_last_error.restype = ctypes.c_char_p
+        lib.oracle_render_bodies.restype = ctypes.c_int
+        lib.oracle_render_bodies.argtypes = [P, P, ctypes.c_size_t, P, P, ctypes.c_int, ctypes.c_int, P]
         _lib = lib
     return _lib
 
@@ -44,8 +37,8 @@ def render(sim, blob, bodies, cam, width, height):
     bodies = np.ascontiguousarray(bodies, np.float64).reshape(sim.num_envs, 11, 9)
     out = np.zeros((sim.num_envs, height, width, 3), np.uint8)
     c = camera(**cam)
-    rc = lib.dfr_render(sim.handle, blob.ctypes.data, blob.nbytes, bodies.ctypes.data, ctypes.addressof(c), int(width), int(height),
-                        out.ctypes.data)
+    rc = lib.oracle_render_bodies(sim.handle, blob.ctypes.data, blob.nbytes, bodies.ctypes.data, ctypes.addressof(c), int(width), int(height),
+                                  out.ctypes.data)
     if rc:
-        raise RenderError(lib.dfr_last_error().decode())
+        raise RenderError(lib.srl_sim_last_error().decode())
     return out

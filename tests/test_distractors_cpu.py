@@ -196,13 +196,19 @@ def test_placement_follows_the_reference_rule(dref):
         assert B[10, 13] == 3 and B[10, 14] == 1
 
 
-def test_cuda_library_exports_set_distractors():
+def test_both_libraries_export_set_distractors(oracle_lib):
     from srl_sim import _abi
+    from srl_sim.model import load_kuka_scene
     path = os.path.join(PKG, "csrc", "libsrl_sim_b200.so")
     if not os.path.isfile(path):
         pytest.fail("%s has not been built (python __graft_entry__.py build)" % path)
-    assert "srl_sim_set_distractors" in _abi.SimLibrary(path).optional
-    assert "srl_sim_set_distractors" in _abi.EXPORTED_SYMBOLS
+    assert "srl_sim_set_distractors" in _abi.EXPORTED_SYMBOLS    # required: SimLibrary refuses a library without it
+    assert hasattr(_abi.SimLibrary(path).lib, "srl_sim_set_distractors")
+    # the oracle exports it too, and refuses: it has no body dynamics
+    sim = _abi.Sim(oracle_lib, "KukaRandButtonGymEnv-v0", 1, -1, model_blob=load_kuka_scene().blob)
+    with pytest.raises(_abi.SimError, match="no distractor body dynamics"):
+        sim.set_distractors(distractor_blob())
+    sim.close()
 
 
 def test_asset_blob_layout():

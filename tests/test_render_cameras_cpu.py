@@ -1,5 +1,5 @@
 """
-One camera per env (srl_sim_render_cameras) on the CPU checker (tests/host/render_cameras_ref.cpp over oracle/liboracle_sim.so): env i's frame is the frame srl_sim_render gives
+One camera per env (srl_sim_render_cameras) on the CPU checker (oracle/liboracle_sim.so): env i's frame is the frame srl_sim_render gives
 env i through cameras[i], byte for byte; with follow_robot the MobileRobot cameras are placed from each robot's position (the reference's
 first-person camera, mobile_robot_env.py:316-332); and BatchedSRLVecEnv(fpv=True) stacks those frames on the top-down ones.
 """
@@ -66,41 +66,15 @@ def follow_targets(pos, cams):
     return out
 
 
-@pytest.fixture(scope="module")
-def checker_lib():
-    import render_cameras_ref
-    return render_cameras_ref.library()
-
-
-@pytest.fixture(scope="module")
-def checker_backend(checker_lib):
-    from srl_sim.backend import Backend
-    return Backend(checker_lib, -1)
-
-
-@pytest.fixture()
-def use_checker_backend(checker_lib):
-    """Route BatchedSRLVecEnv to the CPU checker for the duration of one test."""
-    from srl_sim import backend
-    backend.use_library(checker_lib, -1)
-    yield
-    backend.use_library(None, None)
-
-
-def test_export_exists(oracle_lib, checker_lib):
+def test_both_libraries_export_render_cameras(oracle_lib):
     assert "srl_sim_render_cameras" in _abi.EXPORTED_SYMBOLS
-    assert "srl_sim_render_cameras" in _abi.SimLibrary(_abi.CUDA_LIBRARY_PATH).optional
-    assert "srl_sim_render_cameras" in checker_lib.optional
-    # the oracle library itself has one camera per batch only: the binding refuses instead of calling a missing symbol
-    sim = _abi.Sim(oracle_lib, "MobileRobotGymEnv-v0", 2, -1)
-    with pytest.raises(_abi.SimError, match="per-env cameras"):
-        sim.render_cameras(camera_array([MOBILE_CAMERA] * 2), False, 16, 16, np.zeros((2, 16, 16, 3), np.uint8))
-    sim.close()
+    for lib in (_abi.SimLibrary(_abi.CUDA_LIBRARY_PATH), oracle_lib):
+        assert hasattr(lib.lib, "srl_sim_render_cameras"), lib.path
 
 
 @pytest.mark.parametrize("env_id", sorted(_abi.ENV_KINDS))
-def test_mixed_cameras_match_single_camera_calls(checker_backend, env_id):
-    be = checker_backend
+def test_mixed_cameras_match_single_camera_calls(oracle_backend, env_id):
+    be = oracle_backend
     n = 5
     sim = mid_episode_sim(be, env_id, n, 15)
     cams = mixed_cameras(env_id, n, seed=len(env_id))
@@ -114,8 +88,8 @@ def test_mixed_cameras_match_single_camera_calls(checker_backend, env_id):
 
 
 @pytest.mark.parametrize("env_id", MOBILE_IDS)
-def test_follow_robot_matches_the_fpv_camera(checker_backend, env_id):
-    be = checker_backend
+def test_follow_robot_matches_the_fpv_camera(oracle_backend, env_id):
+    be = oracle_backend
     n = 4
     sim = mid_episode_sim(be, env_id, n, 20, seed=5)
     pos = sim.get_state(_abi.F_ROBOT_POS)
@@ -134,7 +108,7 @@ def test_follow_robot_matches_the_fpv_camera(checker_backend, env_id):
 
 
 @pytest.mark.parametrize("env_id", MOBILE_IDS)
-def test_batched_fpv_observation(use_checker_backend, checker_backend, env_id):
+def test_batched_fpv_observation(use_oracle_backend, oracle_backend, env_id):
     from srl_sim.vec_env import BatchedSRLVecEnv
     n = 3
     kw = dict(seed=4, srl_model="raw_pixels", random_target=True)
@@ -152,14 +126,14 @@ def test_batched_fpv_observation(use_checker_backend, checker_backend, env_id):
     assert o.shape == (n, 224, 224, 6)
     assert np.array_equal(o[..., :3], o_top)
     pos = venv.sim.get_state(_abi.F_ROBOT_POS)
-    want = single_camera_frames(checker_backend, venv.sim, [mobile_fpv_camera(p) for p in pos], 224, 224)
+    want = single_camera_frames(oracle_backend, venv.sim, [mobile_fpv_camera(p) for p in pos], 224, 224)
     assert np.array_equal(o[..., 3:], want)
     assert np.array_equal(venv.render_tensors(), o)
     assert len(venv.get_images()) == n and venv.get_images()[0].shape == (224, 224, 6)
     venv.close(); top.close()
 
 
-def test_kuka_ignores_fpv(use_checker_backend):
+def test_kuka_ignores_fpv(use_oracle_backend):
     from srl_sim.vec_env import BatchedSRLVecEnv
     venv = BatchedSRLVecEnv("KukaButtonGymEnv-v0", 2, srl_model="raw_pixels", fpv=True)
     assert venv.observation_space.shape == (224, 224, 3)
@@ -167,8 +141,8 @@ def test_kuka_ignores_fpv(use_checker_backend):
     venv.close()
 
 
-def test_refusals_carry_the_library_message(checker_backend):
-    be = checker_backend
+def test_refusals_carry_the_library_message(oracle_backend):
+    be = oracle_backend
     kuka = be.make_sim("KukaButtonGymEnv-v0", 2, model_blob=load_kuka_scene().blob)
     kuka.reset()
     buf = np.zeros((2, 16, 16, 3), np.uint8)
@@ -189,3 +163,25 @@ def test_refusals_carry_the_library_message(checker_backend):
     with pytest.raises(ValueError):
         mob.render_cameras(camera_array([MOBILE_CAMERA] * 3), False, 16, 16, buf)
     kuka.close(); mob.close()
+
+
+def test_single_camera_refusals_are_the_cuda_librarys(oracle_backend):
+    """srl_sim_render refuses what the CUDA library refuses (images over 4096 pixels a side, distance <= 0, fov outside (0, 180)), with
+    its messages: both libraries check the arguments with render_core.h's srl_render_args_error."""
+    import re
+    sim = oracle_backend.make_sim("MobileRobotGymEnv-v0", 2)
+    sim.reset()
+    buf = np.zeros((2, 16, 16, 3), np.uint8)
+    fov = "%g" % np.float32(MOBILE_CAMERA["fov"])
+    for (w, h), cam, msg in (((0, 16), MOBILE_CAMERA, "bad image size 0 x 16"), ((16, 4097), MOBILE_CAMERA, "bad image size 16 x 4097"),
+                             ((4097, 16), MOBILE_CAMERA, "bad image size 4097 x 16"),
+                             ((16, 16), dict(MOBILE_CAMERA, distance=0.0), "bad camera (distance 0, fov %s)" % fov),
+                             ((16, 16), dict(MOBILE_CAMERA, distance=-1.0), "bad camera (distance -1, fov %s)" % fov),
+                             ((16, 16), dict(MOBILE_CAMERA, distance=1.0, fov=0.0), "bad camera (distance 1, fov 0)"),
+                             ((16, 16), dict(MOBILE_CAMERA, distance=1.0, fov=180.0), "bad camera (distance 1, fov 180)"),
+                             ((16, 16), dict(MOBILE_CAMERA, distance=float("nan")), "bad camera (distance nan, fov %s)" % fov)):
+        with pytest.raises(_abi.SimError, match=re.escape("srl_sim_render failed (rc=1): render: " + msg) + "$"):
+            sim.render(camera(**cam), w, h, buf)
+    sim.render(camera(**dict(MOBILE_CAMERA, distance=1.0, fov=179.0)), 16, 16, buf)    # the edges of what is accepted
+    sim.render(camera(**MOBILE_CAMERA), 4096, 1, np.zeros((2, 1, 4096, 3), np.uint8))
+    sim.close()

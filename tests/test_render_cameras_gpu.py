@@ -1,5 +1,5 @@
 """
-One camera per env (srl_sim_render_cameras) on the sm_90a library: the per-env path (prepare_cams_kernel, raster_cams_kernel and, with
+One camera per env (srl_sim_render_cameras) on the sm_90a library: the per-env path (prepare_kernel<true>, raster_kernel<..., true> and, with
 follow_robot, follow_cams_kernel) gives env i the bytes srl_sim_render(cameras[i]) gives it on the same handle, at every size, batch size and
 registry id; the camera cache never serves stale cameras; and BatchedSRLVecEnv(fpv=True) renders the first-person frames of a full batch.
 """
@@ -140,14 +140,12 @@ def test_culling_never_changes_a_byte(cuda_backend, env_id, monkeypatch):
 
 
 @pytest.mark.parametrize("env_id", sorted(_abi.ENV_KINDS))
-def test_cuda_per_env_cameras_match_the_cpu_checker(cuda_backend, env_id):
+def test_cuda_per_env_cameras_match_the_cpu_checker(cuda_backend, oracle_backend, env_id):
     """float32 kernel state vs float64 oracle state: silhouette pixels may fall on the other side of an edge, so >= 99.5 % of the bytes."""
-    import render_cameras_ref
-    from srl_sim.backend import Backend
     n = 6
     cams = mixed_cameras(env_id, n, seed=4)
     frames = {}
-    for tag, be in (("cuda", cuda_backend), ("oracle", Backend(render_cameras_ref.library(), -1))):
+    for tag, be in (("cuda", cuda_backend), ("oracle", oracle_backend)):
         sim = mid_episode_sim(be, env_id, n, 12, seed=3)
         out = [be.to_host(render_cameras(sim, be, cams)).copy(), be.to_host(render_cameras(sim, be, cams, width=50, height=33)).copy()]
         if env_id.startswith("Mobile"):

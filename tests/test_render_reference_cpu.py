@@ -167,13 +167,6 @@ def env_cameras(env_id):
     return [KUKA_CAMERA, KUKA_CAMERA_2] if env_id.startswith("Kuka") else [MOBILE_CAMERA]
 
 
-@pytest.fixture(scope="module")
-def checker_backend():
-    import render_cameras_ref
-    from srl_sim.backend import Backend
-    return Backend(render_cameras_ref.library(), -1)
-
-
 @pytest.mark.parametrize("env_id", ENV_IDS)
 def test_checker_frames_match_the_reference(oracle_backend, env_id):
     """Mid-episode and (except MobileRobot2Target, whose redrawn targets get_state cannot show) after an auto-reset: the env cameras at
@@ -196,10 +189,10 @@ def test_checker_frames_match_the_reference(oracle_backend, env_id):
 
 @pytest.mark.parametrize("env_id", ["KukaButtonGymEnv-v0", "Kuka2ButtonGymEnv-v0", "MobileRobotGymEnv-v0", "MobileRobot2TargetGymEnv-v0",
                                     "MobileRobotLineTargetGymEnv-v0"])
-def test_per_env_camera_checker_matches_the_reference(checker_backend, env_id):
-    """The per-env path's checker (tests/host/render_cameras_ref.cpp): one sweep camera per env, odd sizes; MobileRobot with follow_robot
+def test_per_env_camera_checker_matches_the_reference(oracle_backend, env_id):
+    """The checker's per-env path (srl_sim_render_cameras): one sweep camera per env, odd sizes; MobileRobot with follow_robot
     (target float32(float64 position + offset))."""
-    be = checker_backend
+    be = oracle_backend
     n = 4
     sim, targets = make_sim(be, env_id, n, 6, seed=2)
     st = R.read_state(sim, env_id)
@@ -235,7 +228,7 @@ def random_bodies(n, seed):
 
 
 def test_checker_frames_with_bodies_match_the_reference(oracle_backend):
-    """KukaRandButton with caller-given bodies (the oracle has no body dynamics: tests/host/distractor_frames_ref.cpp draws them), both env
+    """KukaRandButton with caller-given bodies (the oracle has no body dynamics: oracle_render_bodies draws them), both env
     cameras and close sweep cameras, mid-episode and after an auto-reset."""
     import distractor_frames_ref as dfr
     env_id = "KukaRandButtonGymEnv-v0"
