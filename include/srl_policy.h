@@ -10,6 +10,8 @@
  *   srl_ppo2_grad   <- the loss + `tf.gradients` of stable-baselines 2.5 `PPO2.setup_model`, run once per minibatch by `PPO2._train_step`
  *   srl_obs_filter  <- stable-baselines `VecNormalize._obfilt` (norm_obs=True, clip_obs=10), wrapped around the envs
  *                      by rl_baselines/utils.py:224-227: running mean / variance update + normalisation
+ *   srl_obs_stack_filter <- `VecFrameStack(envs, num_stack)` -> `VecNormalize` (rl_baselines/utils.py:222-227): the frame stack
+ *                      step and the filter of the stacked rows in one launch
  *
  * Conventions are those of srl_sim.h: 0 on success, message from srl_sim_last_error(); all pointers are DEVICE pointers;
  * calls are asynchronous on `stream` and capturable into a CUDA graph (everything a launch reads that changes between
@@ -29,7 +31,7 @@ extern "C" {
  * Weights in torch.nn.Linear layout: weight [out][in] row-major float32, bias [out]. */
 typedef struct srl_mlp_policy {
     uint32_t struct_size;   /* = sizeof(srl_mlp_policy); checked                          */
-    int32_t  obs_dim;       /* 1..8                                                       */
+    int32_t  obs_dim;       /* 1..32 (1..8 and 9..32 run separate kernel instantiations)  */
     int32_t  n_out;         /* Discrete: number of actions (2..8); Box: action dim (1..8) */
     int32_t  discrete;      /* 1 = Categorical(logits), 0 = Normal(mean, exp(logstd))     */
     const float *pi_w1, *pi_b1, *pi_w2, *pi_b2, *pi_w3, *pi_b3;
@@ -55,6 +57,17 @@ int srl_policy_act(const srl_mlp_policy* policy, int n, const float* obs, uint64
 int srl_obs_filter(int n, int obs_dim, const float* obs_raw, double* state, int update, float clip, float eps,
                    float* obs_norm_out, void* stream);
 
+/* VecFrameStack (stable-baselines 2.5) followed by VecNormalize's filter of the stacked rows, in one launch.  W = obs_dim * num_stack,
+ * 1 <= W <= 32; rows are oldest frame first.
+ *   obs_raw : f32[n, obs_dim], the observation of this step (for a done env: the first one of its next episode)
+ *   done    : nullable u8[n]; NULL means reset: every row starts from zeros
+ *   stack   : f32[n, W], updated in place: roll left by obs_dim, zero the row where done[i] != 0 (every row when done is NULL), write
+ *             obs_raw into the last obs_dim columns
+ *   state   : f64[2 * W + 1] {mean[W], var[W], count}; update != 0 folds the new stack rows (zeros included) into it first
+ *   obs_norm_out : f32[n, W] = clip((stack - mean) / sqrt(var + eps), -clip, clip), as srl_obs_filter computes it */
+int srl_obs_stack_filter(int n, int obs_dim, int num_stack, const float* obs_raw, const uint8_t* done, float* stack, double* state, int update,
+                         float clip, float eps, float* obs_norm_out, void* stream);
+
 /* Gradient tensors of an MlpPolicy, same shapes and layout as the weights (torch: `param.grad`, contiguous float32). */
 typedef struct srl_mlp_grads {
     uint32_t struct_size;   /* = sizeof(srl_mlp_grads); checked */
@@ -76,7 +89,7 @@ typedef struct srl_mlp_grads {
  *   adv, ret, old_logp, old_value : f32[rows]
  *   workspace  : device memory of at least srl_ppo2_workspace_bytes(...) bytes (per-CTA partial gradients; no state between calls)
  * The gradient tensors are OVERWRITTEN (not accumulated).  Deterministic: partial sums are combined in a fixed order. */
-size_t srl_ppo2_workspace_bytes(int obs_dim, int n_out, int discrete, int minibatch);
+size_t srl_ppo2_workspace_bytes(int obs_dim, int n_out, int discrete, int minibatch);   /* 0 for an unsupported shape */
 int srl_ppo2_grad(const srl_mlp_policy* policy, const srl_mlp_grads* grads, int minibatch, const int64_t* idx, const float* obs,
                   const void* actions, const float* adv, const float* ret, const float* old_logp, const float* old_value,
                   float cliprange, float ent_coef, float vf_coef, void* workspace, size_t workspace_bytes, void* stream);

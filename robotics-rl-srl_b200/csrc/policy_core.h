@@ -1,5 +1,6 @@
 // Per-environment arithmetic of the fused PPO2 "policy act" step, shared by the sm_90a kernel (policy_kernels.cu) and by the
-// CPU checker the tests build from it (oracle/policy_ref.cpp) -- plain C++, no CUDA types.
+// CPU checker the tests build from it (oracle/policy_ref.cpp) -- plain C++, no CUDA types.  The checker takes any obs_dim: the
+// tower below reads the observation width at run time, so it covers the narrow (<= 8) and the wide (<= 32) kernels alike.
 //
 // What it computes is what stable-baselines' PPO2 runner does per env step through `model.step(obs)` with `MlpPolicy`
 // (rl_baselines/rl_algorithm/ppo2.py:58-72 of the reference picks that policy): two separate 64-64 tanh towers -- policy logits
@@ -17,6 +18,7 @@
 
 #define SRL_POLICY_HIDDEN 64
 #define SRL_POLICY_MAX_OBS 8
+#define SRL_POLICY_WIDE_OBS 32     // widest observation of the wide kernel instantiations (stacked states); widths above 8 take those
 #define SRL_POLICY_MAX_OUT 8
 enum { SRL_PHILOX_PURPOSE_POLICY = 16 };   // counter word 3 of the policy-sampling stream (the simulator uses 0..10, csrc/philox.cuh)
 

@@ -94,8 +94,14 @@ __device__ __forceinline__ float dot_row(const float* row, const float (&a)[H], 
 // outputs ((t % 16) + 0, 16, 32, 48) -- per 4 inputs it loads 4 weight quads + 4 activation quads (8 LDS.128) for 64 FFMA into 64 independent
 // accumulators.  (One env's 16 outputs per thread needed 1 LDS.128 per 4 FFMA and was bound by the shared-memory pipe: ncu: most of the
 // stalls on the first FFMA after a weight load.)  The 8 lanes of a quarter-warp read 8 consecutive weight
-// rows (stride WS = 68 words: 8 different 4-bank groups) and one common activation quad (broadcast).  `xs` [32][8] observations, `ha` / `hb`
+// rows (stride WS = 68 words: 8 different 4-bank groups) and one common activation quad (broadcast).  `xs` [32][MO] observations, `ha` / `hb`
 // [32][WS] activation columns (layer 1 -> ha, layer 2 -> hb), `out` [32][stride] receives the last layer (thread t: env t / 4, outputs t % 4 + 4 k).
+// MO = SRL_POLICY_MAX_OBS: W1 is [64][D], one input per step.  MO = SRL_POLICY_WIDE_OBS: W1 rows are padded to w1_stride<MO>() = MO + 4 words and
+// both W1 and `xs` rows are zero past D, so layer 1 takes 4 inputs per step (one LDS.128 per weight row and per env) for any D; the FMA chain per
+// output is still d = 0, 1, ... in order, and the padded inputs add 0 * 0.
+template <int MO>
+__host__ __device__ constexpr int w1_stride() { return MO == SRL_POLICY_MAX_OBS ? MO : MO + 4; }
+template <int MO>
 __device__ __forceinline__ void tower_tiled(const TowerSmem& W, int D, int n_out, const float* xs, float* ha, float* hb, float* out, int out_stride) {
     const int t = threadIdx.x, eg = t >> 4, og = t & 15;
     {   // layer 1: obs_dim -> 64
@@ -104,16 +110,33 @@ __device__ __forceinline__ void tower_tiled(const TowerSmem& W, int D, int n_out
         for (int k = 0; k < 4; ++k)
 #pragma unroll
             for (int e = 0; e < 4; ++e) acc[e][k] = W.b1[og + 16 * k];
-        for (int d = 0; d < D; ++d) {
-            float w[4], x[4];
+        if constexpr (MO == SRL_POLICY_MAX_OBS) {
+            for (int d = 0; d < D; ++d) {
+                float w[4], x[4];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) w[k] = W.w1[(og + 16 * k) * D + d];
+                for (int k = 0; k < 4; ++k) w[k] = W.w1[(og + 16 * k) * D + d];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) x[e] = xs[(4 * eg + e) * SRL_POLICY_MAX_OBS + d];
+                for (int e = 0; e < 4; ++e) x[e] = xs[(4 * eg + e) * SRL_POLICY_MAX_OBS + d];
 #pragma unroll
-            for (int e = 0; e < 4; ++e)
+                for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) acc[e][k] = fmaf(w[k], x[e], acc[e][k]);
+                    for (int k = 0; k < 4; ++k) acc[e][k] = fmaf(w[k], x[e], acc[e][k]);
+            }
+        } else {
+            for (int d4 = 0; d4 < D; d4 += 4) {
+                float4 w[4], x[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) w[k] = *reinterpret_cast<const float4*>(W.w1 + (og + 16 * k) * w1_stride<MO>() + d4);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) x[e] = *reinterpret_cast<const float4*>(xs + (4 * eg + e) * MO + d4);
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        acc[e][k] = fmaf(w[k].x, x[e].x, acc[e][k]); acc[e][k] = fmaf(w[k].y, x[e].y, acc[e][k]);
+                        acc[e][k] = fmaf(w[k].z, x[e].z, acc[e][k]); acc[e][k] = fmaf(w[k].w, x[e].w, acc[e][k]);
+                    }
+            }
         }
 #pragma unroll
         for (int e = 0; e < 4; ++e)
@@ -158,21 +181,25 @@ __device__ __forceinline__ void tower_tiled(const TowerSmem& W, int D, int n_out
     }
 }
 
+// MO: the observation width class (SRL_POLICY_MAX_OBS or SRL_POLICY_WIDE_OBS), which sets the stride of the staged observation rows and of W1
+// (tower_tiled); the wide class zero-fills the padding both read.
+template <int MO>
 __global__ void __launch_bounds__(POLICY_BLOCK) policy_act_kernel(const __grid_constant__ PolicyArgs a) {
     extern __shared__ __align__(16) float smem[];
+    constexpr int W1S = w1_stride<MO>();
     const int D = a.p.obs_dim, A = a.p.n_out;
     float* pi_w2 = smem;                 float* vf_w2 = pi_w2 + H * WS;
     float* pi_w3 = vf_w2 + H * WS;       float* vf_w3 = pi_w3 + SRL_POLICY_MAX_OUT * WS;
     float* ha = vf_w3 + WS;              float* hb = ha + POLICY_ENVS * WS;       // [POLICY_ENVS][WS] activation columns (16-byte aligned)
-    float* pi_w1 = hb + POLICY_ENVS * WS;            float* vf_w1 = pi_w1 + H * SRL_POLICY_MAX_OBS;
-    float* pi_b1 = vf_w1 + H * SRL_POLICY_MAX_OBS;   float* vf_b1 = pi_b1 + H;
+    float* pi_w1 = hb + POLICY_ENVS * WS;            float* vf_w1 = pi_w1 + H * W1S;
+    float* pi_b1 = vf_w1 + H * W1S;                  float* vf_b1 = pi_b1 + H;
     float* pi_b2 = vf_b1 + H;            float* vf_b2 = pi_b2 + H;
     float* pi_b3 = vf_b2 + H;            float* vf_b3 = pi_b3 + SRL_POLICY_MAX_OUT;
     float* s_logstd = vf_b3 + 4;         float* outs = s_logstd + SRL_POLICY_MAX_OUT;   // [POLICY_ENVS][SRL_POLICY_MAX_OUT + 1]: logits / mean, value
-    float* xs = outs + POLICY_ENVS * (SRL_POLICY_MAX_OUT + 1);                           // [POLICY_ENVS][SRL_POLICY_MAX_OBS] observations
+    float* xs = outs + POLICY_ENVS * (SRL_POLICY_MAX_OUT + 1);                           // [POLICY_ENVS][MO] observations
     {
         constexpr int W2PER = H * (H / 4) / POLICY_BLOCK, W3PER = (SRL_POLICY_MAX_OUT * (H / 4) + POLICY_BLOCK - 1) / POLICY_BLOCK;
-        constexpr int W1PER = (H * SRL_POLICY_MAX_OBS + POLICY_BLOCK - 1) / POLICY_BLOCK, XPER = (POLICY_ENVS * SRL_POLICY_MAX_OBS + POLICY_BLOCK - 1) / POLICY_BLOCK;
+        constexpr int W1PER = (H * MO + POLICY_BLOCK - 1) / POLICY_BLOCK, XPER = (POLICY_ENVS * MO + POLICY_BLOCK - 1) / POLICY_BLOCK;
         static_assert(H * (H / 4) % POLICY_BLOCK == 0 && H <= POLICY_BLOCK && SRL_POLICY_MAX_OUT <= POLICY_BLOCK, "staging shape");
         const bool vec = ((reinterpret_cast<uintptr_t>(a.p.pi_w2) | reinterpret_cast<uintptr_t>(a.p.vf_w2) | reinterpret_cast<uintptr_t>(a.p.pi_w3) |
                            reinterpret_cast<uintptr_t>(a.p.vf_w3)) & 15u) == 0;
@@ -187,14 +214,26 @@ __global__ void __launch_bounds__(POLICY_BLOCK) policy_act_kernel(const __grid_c
         const int first = blockIdx.x * POLICY_ENVS, nx = min(POLICY_ENVS, a.n - first) * D;
         vec_load(r_x, a.obs + (size_t)first * D, nx);
         rows_store(r_pw2, pi_w2, H); rows_store(r_vw2, vf_w2, H); rows_store(r_pw3, pi_w3, A); rows_store(r_vw3, vf_w3, 1);
-        vec_store(r_pw1, pi_w1, H * D); vec_store(r_vw1, vf_w1, H * D);
+        if constexpr (MO == SRL_POLICY_MAX_OBS) {
+            vec_store(r_pw1, pi_w1, H * D); vec_store(r_vw1, vf_w1, H * D);
+        } else {                                             // [64][D] -> [64][W1S], zero past D (disjoint from the weight stores)
+#pragma unroll
+            for (int k = 0; k < W1PER; ++k) {
+                const int i = threadIdx.x + k * POLICY_BLOCK;
+                if (i < H * D) { pi_w1[(i / D) * W1S + i % D] = r_pw1.v[k]; vf_w1[(i / D) * W1S + i % D] = r_vw1.v[k]; }
+            }
+            for (int j = threadIdx.x; j < H * W1S; j += POLICY_BLOCK)
+                if (j % W1S >= D) { pi_w1[j] = 0.f; vf_w1[j] = 0.f; }
+            for (int j = threadIdx.x; j < POLICY_ENVS * MO; j += POLICY_BLOCK)
+                if (j % MO >= D) xs[j] = 0.f;
+        }
         vec_store(r_pb1, pi_b1, H); vec_store(r_vb1, vf_b1, H); vec_store(r_pb2, pi_b2, H); vec_store(r_vb2, vf_b2, H);
         vec_store(r_pb3, pi_b3, A); vec_store(r_vb3, vf_b3, 1);
         vec_store(r_ls, s_logstd, a.p.discrete ? 0 : A);
 #pragma unroll
         for (int k = 0; k < XPER; ++k) {                     // [env][D] -> [env][8]; envs past n read as zeros (their results are never stored)
             const int j = threadIdx.x + k * POLICY_BLOCK;
-            if (j < POLICY_ENVS * D) xs[(j / D) * SRL_POLICY_MAX_OBS + (j % D)] = r_x.v[k];
+            if (j < POLICY_ENVS * D) xs[(j / D) * MO + (j % D)] = r_x.v[k];
             if (a.obs_buf && j < nx) a.obs_buf[(size_t)first * D + j] = r_x.v[k];
         }
     }
@@ -202,8 +241,8 @@ __global__ void __launch_bounds__(POLICY_BLOCK) policy_act_kernel(const __grid_c
     __syncthreads();
     const TowerSmem Wpi = {pi_w1, pi_b1, pi_w2, pi_b2, pi_w3, pi_b3};
     const TowerSmem Wvf = {vf_w1, vf_b1, vf_w2, vf_b2, vf_w3, vf_b3};
-    tower_tiled(Wpi, D, A, xs, ha, hb, outs, SRL_POLICY_MAX_OUT + 1);
-    tower_tiled(Wvf, D, 1, xs, ha, hb, outs + SRL_POLICY_MAX_OUT, SRL_POLICY_MAX_OUT + 1);   // its layer 1 rewrites `ha`, last read before the previous tower's second barrier
+    tower_tiled<MO>(Wpi, D, A, xs, ha, hb, outs, SRL_POLICY_MAX_OUT + 1);
+    tower_tiled<MO>(Wvf, D, 1, xs, ha, hb, outs + SRL_POLICY_MAX_OUT, SRL_POLICY_MAX_OUT + 1);   // its layer 1 rewrites `ha`, last read before the previous tower's second barrier
     __syncwarp();                                            // an env's outputs were written by the 4 lanes t / 4 = env of this warp
     const int slot = threadIdx.x >> 2, u = threadIdx.x & 3;
     const int i = blockIdx.x * POLICY_ENVS + slot;
@@ -331,9 +370,86 @@ __global__ void __launch_bounds__(FILTER_BLOCK) obs_filter_kernel(int n, const f
     }
 }
 
+// VecFrameStack + VecNormalize in one CTA: advance the caller's [n][W = k D] stack by the new observation, then filter the W-wide rows like
+// obs_filter_kernel does (one pass about the running mean m0, float64 sums, the same merge and normalisation).  Thread t owns column t % W of
+// rows t / W + R u (R = FILTER_BLOCK / W rows per slot, STACK_ROWS slots per pass): its sums are those of one column, so a column's total is one
+// warp's reduction over the R threads of that column (W <= 32 = the number of warps).  The roll reads column c + D of the row it writes, which
+// another thread of the same pass overwrites: every load of a pass precedes the barrier, every store follows it.  The second sweep re-reads
+// the stack (L2-resident at the trainer's sizes): W <= 32 columns per row do not fit in registers the way obs_filter_kernel's <= 8 do.
+constexpr int STACK_ROWS = 8;
+__global__ void __launch_bounds__(FILTER_BLOCK) obs_stack_filter_kernel(int n, int D, int K, const float* __restrict__ obs, const uint8_t* __restrict__ done,
+                                                                         float* stack, double* state, int update, float clip, float eps,
+                                                                         float* __restrict__ out) {
+    __shared__ double red[2][FILTER_BLOCK];
+    __shared__ float s_mf[SRL_POLICY_WIDE_OBS], s_inv[SRL_POLICY_WIDE_OBS];
+    const int W = D * K, keep = W - D, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int R = FILTER_BLOCK / W, r = tid / W, c = tid - r * W;
+    const bool active = r < R;
+    const double m0 = (update && active) ? state[c] : 0.0;
+    double s1 = 0.0, s2 = 0.0;
+    for (int base = 0; base < n; base += R * STACK_ROWS) {
+        float v[STACK_ROWS];
+#pragma unroll
+        for (int u = 0; u < STACK_ROWS; ++u) {
+            const int i = base + r + R * u;
+            v[u] = 0.f;
+            if (active && i < n) {
+                if (c >= keep) v[u] = obs[(size_t)i * D + (c - keep)];                      // the newest frame: the last D columns
+                else if (done && !done[i]) v[u] = stack[(size_t)i * W + c + D];           // roll left by D; a done env (or a reset: done == NULL) starts from zeros
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int u = 0; u < STACK_ROWS; ++u) {
+            const int i = base + r + R * u;
+            if (active && i < n) {
+                stack[(size_t)i * W + c] = v[u];
+                const double d = (double)v[u] - m0;
+                s1 += d; s2 = fma(d, d, s2);
+            }
+        }
+    }
+    if (update) {
+        red[0][tid] = s1; red[1][tid] = s2;
+        __syncthreads();
+        if (warp < W) {                  // warp w: column w, summed over the R threads that own it
+            double a1 = 0.0, a2 = 0.0;
+            for (int q = lane; q < R; q += 32) { a1 += red[0][q * W + warp]; a2 += red[1][q * W + warp]; }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) { a1 += __shfl_xor_sync(0xffffffffu, a1, o); a2 += __shfl_xor_sync(0xffffffffu, a2, o); }
+            if (lane == 0) {
+                const int d = warp;
+                const double count = state[2 * W], bc = (double)n, tot = count + bc;
+                const double b1 = a1 / bc, bmean = state[d] + b1, bvar = a2 / bc - b1 * b1;
+                const double mean = state[d], var = state[W + d], delta = bmean - mean;
+                const double nm = mean + delta * bc / tot, nv = (var * count + bvar * bc + delta * delta * count * bc / tot) / tot;
+                state[d] = nm; state[W + d] = nv;
+                s_mf[d] = (float)nm; s_inv[d] = sqrtf((float)nv + eps);
+            }
+        }
+        __syncthreads();                 // every column's lane 0 has read the count before thread 0 moves it
+        if (tid == 0) state[2 * W] += (double)n;
+    } else {
+        if (tid < W) { s_mf[tid] = (float)state[tid]; s_inv[tid] = sqrtf((float)state[W + tid] + eps); }
+        __syncthreads();                 // also orders the stack stores above before the reads below
+    }
+    const size_t total = (size_t)n * W;
+    for (size_t e0 = tid; e0 < total; e0 += (size_t)4 * FILTER_BLOCK) {
+        float x[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) { const size_t e = e0 + (size_t)u * FILTER_BLOCK; x[u] = e < total ? stack[e] : 0.f; }
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const size_t e = e0 + (size_t)u * FILTER_BLOCK;
+            if (e < total) { const int col = (int)(e % (size_t)W); out[e] = fminf(fmaxf((x[u] - s_mf[col]) / s_inv[col], -clip), clip); }
+        }
+    }
+}
+
+template <int MO>
 constexpr size_t policy_smem_bytes() {
-    return sizeof(float) * (size_t)(2 * H * WS + SRL_POLICY_MAX_OUT * WS + WS + 2 * POLICY_ENVS * WS + 2 * H * SRL_POLICY_MAX_OBS + 4 * H + SRL_POLICY_MAX_OUT + 4 +
-                                    SRL_POLICY_MAX_OUT + POLICY_ENVS * (SRL_POLICY_MAX_OUT + 1) + POLICY_ENVS * SRL_POLICY_MAX_OBS);
+    return sizeof(float) * (size_t)(2 * H * WS + SRL_POLICY_MAX_OUT * WS + WS + 2 * POLICY_ENVS * WS + 2 * H * w1_stride<MO>() + 4 * H + SRL_POLICY_MAX_OUT + 4 +
+                                    SRL_POLICY_MAX_OUT + POLICY_ENVS * (SRL_POLICY_MAX_OUT + 1) + POLICY_ENVS * MO);
 }
 
 }  // namespace
@@ -345,17 +461,25 @@ int srl_policy_act(const srl_mlp_policy* p, int n, const float* obs, uint64_t* r
     if (!p || !obs || !rng || !act_env || !logp || !value) { srl_set_error("policy_act: null argument"); return 1; }
     if (p->struct_size != sizeof(srl_mlp_policy)) { srl_set_error("policy_act: srl_mlp_policy size mismatch (%u != %zu)", p->struct_size, sizeof(srl_mlp_policy)); return 1; }
     if (n <= 0) { srl_set_error("policy_act: n must be positive"); return 1; }
-    if (p->obs_dim < 1 || p->obs_dim > SRL_POLICY_MAX_OBS || p->n_out < 1 || p->n_out > SRL_POLICY_MAX_OUT || (p->discrete && p->n_out < 2)) {
-        srl_set_error("policy_act: unsupported shape obs_dim=%d n_out=%d", p->obs_dim, p->n_out); return 1;
+    if (p->obs_dim < 1 || p->obs_dim > SRL_POLICY_WIDE_OBS || p->n_out < 1 || p->n_out > SRL_POLICY_MAX_OUT || (p->discrete && p->n_out < 2)) {
+        srl_set_error("policy_act: unsupported shape obs_dim=%d n_out=%d (obs_dim 1..%d, n_out 1..%d)", p->obs_dim, p->n_out, SRL_POLICY_WIDE_OBS,
+                      SRL_POLICY_MAX_OUT); return 1;
     }
     if (!p->pi_w1 || !p->pi_b1 || !p->pi_w2 || !p->pi_b2 || !p->pi_w3 || !p->pi_b3 || !p->vf_w1 || !p->vf_b1 || !p->vf_w2 || !p->vf_b2 ||
         !p->vf_w3 || !p->vf_b3 || (!p->discrete && !p->logstd)) { srl_set_error("policy_act: null weight pointer"); return 1; }
-    constexpr size_t smem = policy_smem_bytes();
-    SRL_CUDA_OK(srl_smem_opt_in<policy_act_kernel>(smem));
     PolicyArgs a;
     a.p = *p; a.n = n; a.obs = obs; a.rng = reinterpret_cast<unsigned long long*>(rng); a.env_offset = env_offset;
     a.obs_buf = obs_buf; a.act_env = act_env; a.act_buf = act_buf; a.logp = logp; a.value = value;
-    policy_act_kernel<<<(n + POLICY_ENVS - 1) / POLICY_ENVS, POLICY_BLOCK, smem, (cudaStream_t)stream>>>(a);
+    const int grid = (n + POLICY_ENVS - 1) / POLICY_ENVS;
+    if (p->obs_dim <= SRL_POLICY_MAX_OBS) {
+        constexpr size_t smem = policy_smem_bytes<SRL_POLICY_MAX_OBS>();
+        SRL_CUDA_OK(srl_smem_opt_in<policy_act_kernel<SRL_POLICY_MAX_OBS>>(smem));
+        policy_act_kernel<SRL_POLICY_MAX_OBS><<<grid, POLICY_BLOCK, smem, (cudaStream_t)stream>>>(a);
+    } else {
+        constexpr size_t smem = policy_smem_bytes<SRL_POLICY_WIDE_OBS>();
+        SRL_CUDA_OK(srl_smem_opt_in<policy_act_kernel<SRL_POLICY_WIDE_OBS>>(smem));
+        policy_act_kernel<SRL_POLICY_WIDE_OBS><<<grid, POLICY_BLOCK, smem, (cudaStream_t)stream>>>(a);
+    }
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -370,6 +494,19 @@ int srl_obs_filter(int n, int obs_dim, const float* obs_raw, double* state, int 
 #undef SRL_FILTER_CASE
         default: srl_set_error("obs_filter: unsupported obs_dim %d", obs_dim); return 1;
     }
+    SRL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int srl_obs_stack_filter(int n, int obs_dim, int num_stack, const float* obs_raw, const uint8_t* done, float* stack, double* state, int update,
+                         float clip, float eps, float* obs_norm_out, void* stream) {
+    if (!obs_raw || !stack || !state || !obs_norm_out) { srl_set_error("obs_stack_filter: null argument"); return 1; }
+    if (n <= 0 || obs_dim < 1 || num_stack < 1 || obs_dim > SRL_POLICY_WIDE_OBS || num_stack > SRL_POLICY_WIDE_OBS || obs_dim * num_stack > SRL_POLICY_WIDE_OBS) {
+        srl_set_error("obs_stack_filter: unsupported shape n=%d obs_dim=%d num_stack=%d (obs_dim * num_stack must be 1..%d)", n, obs_dim, num_stack,
+                      SRL_POLICY_WIDE_OBS);
+        return 1;
+    }
+    obs_stack_filter_kernel<<<1, FILTER_BLOCK, 0, (cudaStream_t)stream>>>(n, obs_dim, num_stack, obs_raw, done, stack, state, update, clip, eps, obs_norm_out);
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }

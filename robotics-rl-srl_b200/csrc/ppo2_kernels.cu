@@ -20,6 +20,7 @@
 namespace {
 
 constexpr int H = 64, WS = 68, CH = 64, NT = 256, MAXO = 8, MAXD = 8;      // 64 samples per chunk, 8 warps per CTA (two per scheduler)
+constexpr int WIDE_D = 32;     // the wide instantiation: observation widths 9..32 (stacked states)
 static_assert(NT == 4 * CH && NT == 256, "thread roles: 4 threads per sample in the heads, 128 owners per tower of the W2 gradient patches");
 
 // offsets of the parameter tensors inside a flat gradient vector (the order of the per-CTA partials)
@@ -107,12 +108,15 @@ __device__ __forceinline__ float dot64(const float* row, const float* col) {
 
 struct SampleRegs { float x[MAXD], af[MAXO], adv, ret, olp, ov; int ai, valid; };
 
+template <bool LOAD_X>
 __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs& r) {
     const int D = a.p.obs_dim, A = a.p.n_out;
     r.valid = s < a.mb;
     const long long g = r.valid ? (a.idx ? a.idx[s] : (long long)s) : 0;
+    if constexpr (LOAD_X) {
 #pragma unroll
-    for (int d = 0; d < MAXD; ++d) r.x[d] = (r.valid && d < D) ? a.obs[g * D + d] : 0.f;
+        for (int d = 0; d < MAXD; ++d) r.x[d] = (r.valid && d < D) ? a.obs[g * D + d] : 0.f;
+    }
     r.ai = 0;
 #pragma unroll
     for (int k = 0; k < MAXO; ++k) r.af[k] = 0.f;
@@ -126,7 +130,29 @@ __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs
     r.adv = r.valid ? a.adv[g] : 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = r.valid ? a.old_logp[g] : 0.f; r.ov = r.valid ? a.old_val[g] : 0.f;
 }
 
-__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) {
+// The wide instantiation (MD = WIDE_D) differs from the narrow one (MD = MAXD) in three places, all to fit shared memory and registers:
+//  - W1 rows are padded to MD + 1 words (the 16 units a layer-1 step reads sit in 16 different banks), `xs` rows are MD wide;
+//  - a chunk's observation rows are prefetched by all 256 threads (thread t: sample t / 4, columns t % 4 + 4 j), 8 registers each, instead of
+//    a [MD] array in the 64 sample threads' SampleRegs (32 more registers there would spill);
+//  - the first-layer deltas d1 overwrite the second-layer activations hb, which are dead once the layer-3 gradients are taken: one more barrier
+//    per chunk, 34 KB less shared memory (the wider W1 copies and rows need 18 KB more than the narrow kernel's 224 KB leave).
+// the wide kernel's observation prefetch: columns u + 4 j (j < XQ) of sample s, zero past D and past the minibatch
+template <int XQ>
+__device__ __forceinline__ void load_row_part(const GradArgs& a, int s, int u, float (&x)[XQ]) {
+    const int D = a.p.obs_dim;
+    const bool valid = s < a.mb;
+    const long long g = valid ? (a.idx ? a.idx[s] : (long long)s) : 0;
+#pragma unroll
+    for (int j = 0; j < XQ; ++j) x[j] = (valid && u + 4 * j < D) ? a.obs[g * D + u + 4 * j] : 0.f;
+}
+
+template <int MD>
+__host__ __device__ constexpr int grad_w1_stride() { return MD == MAXD ? MAXD : MD + 1; }
+template <int MD>
+__device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
+    constexpr bool WIDE = MD != MAXD;
+    constexpr int W1S = grad_w1_stride<MD>(), XQ = MD / 4;     // XQ: observation columns per thread of the wide prefetch
+    constexpr int G1 = WIDE ? (H * MD) / NT : 4;              // W1 gradient entries per thread
     extern __shared__ __align__(16) float sm[];
     const int D = a.p.obs_dim, A = a.p.n_out, t = threadIdx.x;
     const bool discrete = a.p.discrete != 0;
@@ -135,12 +161,13 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
     float* w2p = sm;                 float* w2v = w2p + H * WS;       float* w2pT = w2v + H * WS;      float* w2vT = w2pT + H * WS;
     float* w3p = w2vT + H * WS;      float* w3v = w3p + MAXO * WS;
     float* hap = w3v + WS;           float* hbp = hap + CH * WS;      float* hav = hbp + CH * WS;      float* hbv = hav + CH * WS;
-    float* d2p = hbv + CH * WS;      float* d2v = d2p + CH * WS;      float* d1p = d2v + CH * WS;      float* d1v = d1p + CH * WS;
-    float* w1p = d1v + CH * WS;      float* w1v = w1p + H * MAXD;
-    float* b1p = w1v + H * MAXD;     float* b1v = b1p + H;            float* b2p = b1v + H;            float* b2v = b2p + H;
+    float* d2p = hbv + CH * WS;      float* d2v = d2p + CH * WS;
+    float* d1p = WIDE ? hbp : d2v + CH * WS;                          float* d1v = WIDE ? hbv : d1p + CH * WS;
+    float* w1p = WIDE ? d2v + CH * WS : d1v + CH * WS;                float* w1v = w1p + H * W1S;
+    float* b1p = w1v + H * W1S;      float* b1v = b1p + H;            float* b2p = b1v + H;            float* b2v = b2p + H;
     float* b3p = b2v + H;            float* b3v = b3p + MAXO;         float* lsd = b3v + 4;            // logstd
-    float* xs = lsd + MAXO;          // [CH][MAXD]
-    float* zo = xs + CH * MAXD;      // [CH][MAXO + 1]: logits / mean, value at [MAXO]
+    float* xs = lsd + MAXO;          // [CH][MD]
+    float* zo = xs + CH * MD;        // [CH][MAXO + 1]: logits / mean, value at [MAXO]
     float* d3 = zo + CH * (MAXO + 1);   // [CH][MAXO + 1]: d loss / d logits, d loss / d value
     float* dls = d3 + CH * (MAXO + 1);  // [CH][MAXO]: per-sample d loss / d logstd
     float* saf = dls + CH * MAXO;    // [CH][MAXO] actions (Box)
@@ -157,7 +184,7 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
         w3v[e] = a.p.vf_w3[e];
         b1p[e] = a.p.pi_b1[e]; b1v[e] = a.p.vf_b1[e]; b2p[e] = a.p.pi_b2[e]; b2v[e] = a.p.vf_b2[e];
     }
-    for (int e = t; e < H * D; e += NT) { w1p[(e / D) * MAXD + e % D] = a.p.pi_w1[e]; w1v[(e / D) * MAXD + e % D] = a.p.vf_w1[e]; }
+    for (int e = t; e < H * D; e += NT) { w1p[(e / D) * W1S + e % D] = a.p.pi_w1[e]; w1v[(e / D) * W1S + e % D] = a.p.vf_w1[e]; }
     if (t < A) { b3p[t] = a.p.pi_b3[t]; lsd[t] = discrete ? 0.f : a.p.logstd[t]; }
     if (t == 0) b3v[0] = a.p.vf_b3[0];
     __shared__ float s_adv[2];
@@ -181,22 +208,33 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
     for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
         for (int ii = 0; ii < 8; ++ii) gw2[jj][ii] = 0.f;
-    float gw3p[4] = {0.f, 0.f, 0.f, 0.f}, gw1p[4] = {0.f, 0.f, 0.f, 0.f}, gw1v[4] = {0.f, 0.f, 0.f, 0.f};
+    float gw3p[4] = {0.f, 0.f, 0.f, 0.f}, gw1p[G1], gw1v[G1];
+#pragma unroll
+    for (int m = 0; m < G1; ++m) { gw1p[m] = 0.f; gw1v[m] = 0.f; }
     float gw3v = 0.f, gb3 = 0.f, gls = 0.f, gb2 = 0.f, gb1 = 0.f;       // gb2 / gb1: t < 64 the policy tower's unit t, t >= 64 the value tower's unit t - 64
     const int nchunks = (a.mb + CH - 1) / CH;
     SampleRegs cur;
-    if (t < CH) load_sample(a, blockIdx.x * CH + t, cur);
+    float xr[XQ];                                // wide: this thread's columns t % 4 + 4 j of sample t / 4 of the next chunk
+    if (t < CH) load_sample<!WIDE>(a, blockIdx.x * CH + t, cur);
+    if constexpr (WIDE) load_row_part<XQ>(a, blockIdx.x * CH + (t >> 2), t & 3, xr);
     __syncthreads();
     for (int c = blockIdx.x; c < nchunks; c += gridDim.x) {
         // ---- 0: this chunk's samples -> shared; the next chunk's loads are issued now and consumed an iteration later ----
         if (t < CH) {
+            if constexpr (!WIDE) {
 #pragma unroll
-            for (int d = 0; d < MAXD; ++d) xs[t * MAXD + d] = cur.x[d];
+                for (int d = 0; d < MAXD; ++d) xs[t * MAXD + d] = cur.x[d];
+            }
 #pragma unroll
             for (int k = 0; k < MAXO; ++k) saf[t * MAXO + k] = cur.af[k];
             ssc[t * 4] = cur.adv; ssc[t * 4 + 1] = cur.ret; ssc[t * 4 + 2] = cur.olp; ssc[t * 4 + 3] = cur.ov;
             sai[t * 2] = cur.ai; sai[t * 2 + 1] = cur.valid;
-            load_sample(a, (c + gridDim.x) * CH + t, cur);
+            load_sample<!WIDE>(a, (c + gridDim.x) * CH + t, cur);
+        }
+        if constexpr (WIDE) {
+#pragma unroll
+            for (int j = 0; j < XQ; ++j) xs[(t >> 2) * MD + (t & 3) + 4 * j] = xr[j];
+            load_row_part<XQ>(a, (c + gridDim.x) * CH + (t >> 2), t & 3, xr);
         }
         __syncthreads();
         // ---- 1: forward, both towers ----
@@ -209,9 +247,9 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
             for (int d = 0; d < D; ++d) {
                 float wp[4], wv[4], x[4];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { wp[k] = w1p[(og + 16 * k) * MAXD + d]; wv[k] = w1v[(og + 16 * k) * MAXD + d]; }
+                for (int k = 0; k < 4; ++k) { wp[k] = w1p[(og + 16 * k) * W1S + d]; wv[k] = w1v[(og + 16 * k) * W1S + d]; }
 #pragma unroll
-                for (int e = 0; e < 4; ++e) x[e] = xs[(4 * eg + e) * MAXD + d];
+                for (int e = 0; e < 4; ++e) x[e] = xs[(4 * eg + e) * MD + d];
 #pragma unroll
                 for (int e = 0; e < 4; ++e)
 #pragma unroll
@@ -383,6 +421,7 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
                         for (int ii = 0; ii < 8; ++ii) gw2[jj][ii] = fmaf(dd[jj], hh[ii], gw2[jj][ii]);
                 }
             }
+            if constexpr (WIDE) __syncthreads();        // d1 overwrites hb: every read of hb above comes first
             // delta 1 = (W2^T delta 2) (1 - h1^2): the same tile as the forward pass, on the transposed weights
             float o[4][4];
             tile_matvec(w2pT, nullptr, d2p, eg, og, o);
@@ -407,13 +446,14 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
                 for (int n = 0; n < CH; ++n) sb += d1[n * WS + unit];
                 gb1 += sb;
             }
-            for (int m = 0; m < 4; ++m) {
+#pragma unroll
+            for (int m = 0; m < G1; ++m) {
                 const int e = t + NT * m;
                 if (e < H * D) {
                     const int i = e / D, d = e % D;
                     float sp = 0.f, sv = 0.f;
 #pragma unroll 8
-                    for (int n = 0; n < CH; ++n) { const float x = xs[n * MAXD + d]; sp = fmaf(d1p[n * WS + i], x, sp); sv = fmaf(d1v[n * WS + i], x, sv); }
+                    for (int n = 0; n < CH; ++n) { const float x = xs[n * MD + d]; sp = fmaf(d1p[n * WS + i], x, sp); sv = fmaf(d1v[n * WS + i], x, sv); }
                     gw1p[m] += sp; gw1v[m] += sv;
                 }
             }
@@ -426,10 +466,22 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
     for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
         for (int ii = 0; ii < 8; ++ii) out[(own_pi ? seg.pw2 : seg.vw2) + (4 * jq + jj) * H + 8 * iq + ii] = gw2[jj][ii];
-    for (int m = 0; m < 4; ++m) {
-        const int e = t + NT * m;
-        if (e < A * H) out[seg.pw3 + e] = gw3p[m];
-        if (e < H * D) { out[seg.pw1 + e] = gw1p[m]; out[seg.vw1 + e] = gw1v[m]; }
+    if constexpr (!WIDE) {
+        for (int m = 0; m < 4; ++m) {
+            const int e = t + NT * m;
+            if (e < A * H) out[seg.pw3 + e] = gw3p[m];
+            if (e < H * D) { out[seg.pw1 + e] = gw1p[m]; out[seg.vw1 + e] = gw1v[m]; }
+        }
+    } else {
+        for (int m = 0; m < 4; ++m) {
+            const int e = t + NT * m;
+            if (e < A * H) out[seg.pw3 + e] = gw3p[m];
+        }
+#pragma unroll
+        for (int m = 0; m < G1; ++m) {
+            const int e = t + NT * m;
+            if (e < H * D) { out[seg.pw1 + e] = gw1p[m]; out[seg.vw1 + e] = gw1v[m]; }
+        }
     }
     if (t < H) { out[seg.vw3 + t] = gw3v; out[seg.pb2 + t] = gb2; out[seg.pb1 + t] = gb1; }
     else if (t < 2 * H) { out[seg.vb2 + (t - H)] = gb2; out[seg.vb1 + (t - H)] = gb1; }
@@ -437,6 +489,9 @@ __global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant_
     if (t == MAXO) out[seg.vb3] = gb3;
     if (!discrete && t >= 16 && t < 16 + A) out[seg.ls + (t - 16)] = gls;
 }
+
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD>(a); }
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D>(a); }
 
 // GAE(lambda) of one rollout, the reference's backward recursion (stable-baselines PPO2 runner): one thread per env, T sequential steps,
 // eight steps' loads in flight.  Separate roundings (no FMA contraction): the same bits as the torch recursion of rl_baselines/ppo2.py.
@@ -488,10 +543,12 @@ __global__ void ppo2_reduce_kernel(const __grid_constant__ ReduceArgs r) {
     dst[off] = s;
 }
 
+template <int MD>
 constexpr size_t grad_smem_bytes() {
-    return sizeof(float) * (size_t)(4 * H * WS + MAXO * WS + WS + 8 * CH * WS + 2 * H * MAXD + 4 * H + MAXO + 4 + MAXO + CH * MAXD + 2 * CH * (MAXO + 1) +
-                                    2 * CH * MAXO + CH * 4 + CH * 2);
+    return sizeof(float) * (size_t)(4 * H * WS + MAXO * WS + WS + (MD == MAXD ? 8 : 6) * CH * WS + 2 * H * grad_w1_stride<MD>() + 4 * H + MAXO + 4 + MAXO +
+                                    CH * MD + 2 * CH * (MAXO + 1) + 2 * CH * MAXO + CH * 4 + CH * 2);
 }
+static_assert(grad_smem_bytes<MAXD>() <= 227 * 1024 && grad_smem_bytes<WIDE_D>() <= 227 * 1024, "shared memory of one CTA");
 
 int grid_ctas(int mb) {
     static int sms[64] = {};
@@ -508,7 +565,11 @@ int grid_ctas(int mb) {
 extern "C" {
 
 size_t srl_ppo2_workspace_bytes(int obs_dim, int n_out, int discrete, int minibatch) {
-    if (obs_dim < 1 || obs_dim > MAXD || n_out < 1 || n_out > MAXO || minibatch < 1) return 0;
+    if (obs_dim < 1 || obs_dim > WIDE_D || n_out < 1 || n_out > MAXO || minibatch < 1) {
+        srl_set_error("ppo2_workspace_bytes: unsupported shape obs_dim=%d n_out=%d minibatch=%d (obs_dim 1..%d, n_out 1..%d)", obs_dim, n_out, minibatch,
+                      WIDE_D, MAXO);
+        return 0;
+    }
     const Seg seg = make_seg(obs_dim, n_out, discrete);
     const int ctas = grid_ctas(minibatch);
     return 2048 + sizeof(float) * (size_t)seg.P * (size_t)(ctas > 0 ? ctas : 1);
@@ -519,8 +580,9 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
                   void* workspace, size_t workspace_bytes, void* stream) {
     if (!p || !grads || !obs || !actions || !adv || !ret || !old_logp || !old_value || !workspace) { srl_set_error("ppo2_grad: null argument"); return 1; }
     if (p->struct_size != sizeof(srl_mlp_policy) || grads->struct_size != sizeof(srl_mlp_grads)) { srl_set_error("ppo2_grad: struct size mismatch"); return 1; }
-    if (p->obs_dim < 1 || p->obs_dim > MAXD || p->n_out < 1 || p->n_out > MAXO || (p->discrete && p->n_out < 2) || minibatch < 1) {
-        srl_set_error("ppo2_grad: unsupported shape obs_dim=%d n_out=%d minibatch=%d", p->obs_dim, p->n_out, minibatch); return 1;
+    if (p->obs_dim < 1 || p->obs_dim > WIDE_D || p->n_out < 1 || p->n_out > MAXO || (p->discrete && p->n_out < 2) || minibatch < 1) {
+        srl_set_error("ppo2_grad: unsupported shape obs_dim=%d n_out=%d minibatch=%d (obs_dim 1..%d, n_out 1..%d)", p->obs_dim, p->n_out, minibatch,
+                      WIDE_D, MAXO); return 1;
     }
     if (!p->pi_w1 || !p->pi_b1 || !p->pi_w2 || !p->pi_b2 || !p->pi_w3 || !p->pi_b3 || !p->vf_w1 || !p->vf_b1 || !p->vf_w2 || !p->vf_b2 || !p->vf_w3 ||
         !p->vf_b3 || (!p->discrete && !p->logstd)) { srl_set_error("ppo2_grad: null weight pointer"); return 1; }
@@ -530,8 +592,6 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
     if (ctas <= 0) { srl_set_error("ppo2_grad: no CUDA device"); return 1; }
     const Seg seg = make_seg(p->obs_dim, p->n_out, p->discrete);
     if (workspace_bytes < 2048 + sizeof(float) * (size_t)seg.P * (size_t)ctas) { srl_set_error("ppo2_grad: workspace too small (srl_ppo2_workspace_bytes)"); return 1; }
-    constexpr size_t smem = grad_smem_bytes();
-    SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_kernel>(smem));
     cudaStream_t st = (cudaStream_t)stream;
     double* stats = reinterpret_cast<double*>(workspace);
     float* partial = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 2048);
@@ -540,7 +600,15 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
     GradArgs a;
     a.p = *p; a.mb = minibatch; a.idx = reinterpret_cast<const long long*>(idx); a.obs = obs; a.act = actions; a.adv = adv; a.ret = ret;
     a.old_logp = old_logp; a.old_val = old_value; a.clip = cliprange; a.ent_coef = ent_coef; a.vf_coef = vf_coef; a.stats = stats; a.partial = partial;
-    ppo2_grad_kernel<<<ctas, NT, smem, st>>>(a);
+    if (p->obs_dim <= MAXD) {
+        constexpr size_t smem = grad_smem_bytes<MAXD>();
+        SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_kernel>(smem));
+        ppo2_grad_kernel<<<ctas, NT, smem, st>>>(a);
+    } else {
+        constexpr size_t smem = grad_smem_bytes<WIDE_D>();
+        SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_wide_kernel>(smem));
+        ppo2_grad_wide_kernel<<<ctas, NT, smem, st>>>(a);
+    }
     SRL_CUDA_OK(cudaGetLastError());
     ReduceArgs r;
     r.g = *grads; r.seg = seg; r.nparts = ctas; r.partial = partial;

@@ -52,9 +52,13 @@ def main(argv=None):
     train_args, load_path, env_kwargs = loadConfigAndSetup(load_args)
     torch.manual_seed(load_args.seed)
     env = BatchedSRLVecEnv(train_args["env"], load_args.num_cpu, seed=load_args.seed, device=load_args.device, **env_kwargs)
-    dev = env.backend.torch_device
+    on_gpu = env.backend.on_gpu
+    dev = env.backend.torch_device if on_gpu else torch.device("cpu")   # device -1: the CPU oracle a test installs (numpy buffers)
+    as_tensor = (lambda x: x) if on_gpu else torch.from_numpy
     D = env.observation_space.shape[0]
-    policy = (MlpPolicy(D, n_actions=env.action_space.n) if env.is_discrete else MlpPolicy(D, action_dim=env.action_space.shape[0])).to(dev)
+    K = int(train_args.get("num_stack", 1))                       # VecFrameStack of the training run (:140)
+    W = K * D
+    policy = (MlpPolicy(W, n_actions=env.action_space.n) if env.is_discrete else MlpPolicy(W, action_dim=env.action_space.shape[0])).to(dev)
     saved = torch.load(load_path, map_location=dev)
     policy.load_state_dict(saved["policy"])
     mean, var = saved["obs_mean"].float().to(dev), saved["obs_var"].float().to(dev)
@@ -63,7 +67,9 @@ def main(argv=None):
         return torch.clamp((o - mean) / torch.sqrt(var + 1e-8), -10.0, 10.0)
 
     env.sim.reset(obs_out=env._obs, stream=env.backend.stream())
-    obs = normalise(env._obs.clone())
+    stack = torch.zeros((load_args.num_cpu, W), device=dev)       # the trainer's frame stack: oldest frame first, zeroed where an episode ended
+    stack[:, W - D:].copy_(as_tensor(env._obs))
+    obs = normalise(stack.clone())
     n_done, returns = 0, []
     with torch.no_grad():
         for _ in range(load_args.num_timesteps):
@@ -73,13 +79,15 @@ def main(argv=None):
             else:
                 a = dist.sample()
             act = a.to(torch.int32) if env.is_discrete else torch.clamp(a, -1, 1).contiguous()
-            o, _, d, ep_ret, _ = env.step_tensors(act)
+            o, _, d, ep_ret, _ = (as_tensor(x) for x in env.step_tensors(act))
             if bool(d.any()):
                 returns.extend(ep_ret[d.bool()].tolist())
                 if len(returns) - n_done > 1:                      # the reference prints whenever more than one episode ended (:327-330)
                     n_done = len(returns)
                     print("{} episodes - Mean reward: {:.2f}".format(n_done, float(np.mean(returns))))
-            obs = normalise(o.clone())
+            stack.copy_(torch.where(d.bool()[:, None], 0.0, torch.roll(stack, -D, 1)))
+            stack[:, W - D:].copy_(o)
+            obs = normalise(stack.clone())
     n_done = len(returns)
     mean_reward = float(np.mean(returns)) if returns else float("nan")
     print("{} episodes - Mean reward: {:.2f}".format(n_done, mean_reward))

@@ -131,7 +131,7 @@ def allreduce_mean_gradients(params, dist, world):
 
 
 def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None, device=0, hyperparams=None, verbose=1, cuda_graph=True,
-          phase_times=None, fused_act=None, prefetch_resets=None, episode_window=40, fused_update=None):
+          phase_times=None, fused_act=None, prefetch_resets=None, episode_window=40, fused_update=None, num_stack=1):
     """PPO2.learn on a BatchedSRLVecEnv.  Returns a history of (timesteps, mean episode return, fps).
 
     ``cuda_graph``: the n_steps-long collection loop (policy forward, action sampling, observation filter, one simulator
@@ -148,6 +148,10 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     ``fused_update`` (default: on whenever the envs live on a GPU): the gradient of a minibatch step comes from the library's
     ``srl_ppo2_grad`` (include/srl_policy.h: forward, PPO2 loss derivative and backward of both towers in one pass, every activation on chip)
     instead of torch autograd over [minibatch, 64] tensors; gradient clipping, the data-parallel all-reduce and Adam stay in torch.
+    ``num_stack``: ``VecFrameStack(envs, num_stack)`` before the filter, as the reference's ``createEnvs`` wraps every env (rl_baselines/utils.py:222-227):
+    the policy, the filter and the rollout buffer see rows of ``num_stack * D`` values, oldest frame first, zeroed where an episode ended.  The
+    stack is a static device buffer; the fused path advances it and filters it in one launch (``srl_obs_stack_filter``), so an env step stays
+    three launches.  The fused kernels take rows of up to 32 values.
     ``phase_times``: optional dict; when given, every update synchronises between its phases and accumulates the wall time of
     ``collect`` / ``gae`` / ``optimise`` in it (a profiling aid: the synchronisations cost throughput)."""
     hp = dict(PPO2_DEFAULTS); hp.update(hyperparams or {})
@@ -172,10 +176,17 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     dev = env.backend.torch_device if on_gpu else torch.device("cpu")
     e_obs, e_rew, e_done, e_ep_ret, e_ep_len = [x if on_gpu else torch.from_numpy(x) for x in (env._obs, env._rew, env._done, env._ep_ret, env._ep_len)]
     D = env.observation_space.shape[0]
+    K = int(num_stack)
+    if K < 1:
+        raise ValueError("num_stack must be >= 1 (got %d)" % K)
+    W = K * D                                  # the width of what the policy sees: the stacked row
+    if W > 32 and ((on_gpu if fused_act is None else fused_act) or (on_gpu if fused_update is None else fused_update)):
+        from srl_sim.policy import MAX_OBS
+        raise ValueError("num_stack=%d x %d-wide observations = %d: the fused policy kernels take at most %d values per row" % (K, D, W, MAX_OBS))
     if env.is_discrete:
-        policy = MlpPolicy(D, n_actions=env.action_space.n).to(dev)
+        policy = MlpPolicy(W, n_actions=env.action_space.n).to(dev)
     else:
-        policy = MlpPolicy(D, action_dim=env.action_space.shape[0]).to(dev)
+        policy = MlpPolicy(W, action_dim=env.action_space.shape[0]).to(dev)
     params = list(policy.parameters())
     if dist is not None:
         for p in params:                      # same seed => same init; the broadcast makes it independent of library versions
@@ -191,23 +202,28 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         opt = torch.optim.Adam(params, lr=lr_t, eps=1e-5, capturable=True)
     else:
         opt = torch.optim.Adam(params, lr=hp["learning_rate"], eps=1e-5)
-    norm = RunningNorm(D, dev)
+    norm = RunningNorm(W, dev)
     n_updates = max(1, int(num_timesteps) // (N * T * world))
     if log_dir and rank == 0:
         os.makedirs(log_dir, exist_ok=True)
         with open(os.path.join(log_dir, "args.json"), "w") as f:       # train.py:282-283
-            json.dump(dict(env=env_id, algo="ppo2", num_cpu=N, num_timesteps=num_timesteps, seed=seed, srl_model="ground_truth", **hp), f)
+            json.dump(dict(env=env_id, algo="ppo2", num_cpu=N, num_timesteps=num_timesteps, seed=seed, srl_model="ground_truth", num_stack=K, **hp), f)
         with open(os.path.join(log_dir, "env_globals.json"), "w") as f:  # train.py:285-315
             json.dump({k: v for k, v in env_kwargs.items() if isinstance(v, (int, float, str, bool))}, f)
     env.sim.reset(obs_out=env._obs, stream=env.backend.stream())
+    row = e_obs                           # what the filter sees: the observation, or the frame stack over it
+    if K > 1:                             # VecFrameStack.reset: zeros, the first observation in the last D columns
+        stack = torch.zeros((N, W), device=dev)
+        stack[:, W - D:].copy_(e_obs)
+        row = stack
     if dist is not None:                   # the reset batch goes through the same merge, so every rank starts from one filter
         prior = (norm.mean.clone(), norm.var.clone(), norm.count.clone())
-        norm.update(e_obs)
+        norm.update(row)
         merge_running_moments(norm, prior, dist.all_reduce, world)
-        obs = norm(e_obs.clone(), update=False)
+        obs = norm(row.clone(), update=False)
     else:
-        obs = norm(e_obs.clone())        # the current (filtered) observation; updated IN PLACE by the collection loop
-    buf = dict(obs=torch.empty((T, N, D), device=dev), act=torch.empty((T, N) if env.is_discrete else (T, N, env.sim.action_dim), device=dev,
+        obs = norm(row.clone())          # the current (filtered) observation; updated IN PLACE by the collection loop
+    buf = dict(obs=torch.empty((T, N, W), device=dev), act=torch.empty((T, N) if env.is_discrete else (T, N, env.sim.action_dim), device=dev,
                                                                        dtype=torch.int64 if env.is_discrete else torch.float32),
                logp=torch.empty((T, N), device=dev), val=torch.empty((T, N), device=dev), rew=torch.empty((T, N), device=dev),
                done=torch.empty((T, N), device=dev), ep_ret=torch.empty((T, N), device=dev), ep_len=torch.zeros((T, N), device=dev, dtype=torch.int32))
@@ -235,7 +251,12 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
                 act_dev = a.to(torch.int32) if env.is_discrete else torch.clamp(a, -1, 1).contiguous()
                 env.step_tensors(act_dev)                                 # one kernel launch, tensors stay on the GPU
                 buf["rew"][t], buf["done"][t], buf["ep_ret"][t], buf["ep_len"][t] = e_rew, e_done.float(), e_ep_ret, e_ep_len
-                obs.copy_(norm(e_obs))
+                if K > 1:                                                 # VecFrameStack.step: roll by one frame, zero where done, newest frame last
+                    stack.copy_(torch.where(e_done.bool()[:, None], 0.0, torch.roll(stack, -D, 1)))
+                    stack[:, W - D:].copy_(e_obs)
+                    obs.copy_(norm(stack))
+                else:
+                    obs.copy_(norm(e_obs))
             last_val.copy_(policy.vf(obs).squeeze(-1))
 
     def collect_fused():
@@ -246,7 +267,10 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
             for t in range(T):
                 fused.act(N, obs, act_dev, buf["logp"][t], buf["val"][t], obs_buf=buf["obs"][t], act_buf=buf["act"][t], stream=st)
                 env.sim.step(act_dev, None, env._obs, buf["rew"][t], done_u8[t], buf["ep_ret"][t], buf["ep_len"][t], stream=st)
-                fused.filter(N, env._obs, obs, update=True, stream=st)
+                if K > 1:
+                    fused.stack_filter(N, env._obs, done_u8[t], stack, obs, update=True, stream=st)
+                else:
+                    fused.filter(N, env._obs, obs, update=True, stream=st)
             buf["done"].copy_(done_u8)
             last_val.copy_(policy.vf(obs).squeeze(-1))
 
@@ -262,10 +286,13 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(3):
-                policy.act(obs); norm(e_obs, update=False)
+                policy.act(obs); norm(row, update=False)
             if fused is not None:         # first launches outside the capture (one-off function attributes); they change nothing that matters:
                 fused.act(N, obs, act_dev, buf["logp"][0], buf["val"][0], stream=env.backend.stream())     # scratch rows, one sampling counter
-                fused.filter(N, env._obs, obs, update=False, stream=env.backend.stream())                   # re-normalises the current observation
+                if K > 1:                 # a copy of the stack and a scratch output: the stack itself must not advance
+                    fused.stack_filter(N, env._obs, done_u8[0], stack.clone(), torch.empty_like(obs), update=False, stream=env.backend.stream())
+                else:
+                    fused.filter(N, env._obs, obs, update=False, stream=env.backend.stream())               # re-normalises the current observation
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()

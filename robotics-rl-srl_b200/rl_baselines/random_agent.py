@@ -7,8 +7,11 @@ import time
 from srl_sim.vec_env import BatchedSRLVecEnv
 
 
-def train(env_id, num_cpu, num_timesteps, seed=0, env_kwargs=None, device=None, verbose=1):
+def train(env_id, num_cpu, num_timesteps, seed=0, env_kwargs=None, device=None, verbose=1, num_stack=1):
     env = BatchedSRLVecEnv(env_id, num_cpu, seed=seed, device=device, **(env_kwargs or {}))
+    if num_stack > 1:                  # the reference's createEnvs stacks for every algorithm (rl_baselines/utils.py:222)
+        from rl_baselines.utils import VecFrameStack
+        env = VecFrameStack(env, num_stack)
     env.action_space.seed(seed)
     env.reset()
     num_updates = int(num_timesteps) // num_cpu

@@ -32,7 +32,7 @@ def main(argv=None):
     parser.add_argument('--env', type=str, help='environment ID', default='KukaButtonGymEnv-v0', choices=list(registered_env.keys()))
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--episode_window', type=int, default=40, help='Episode window for moving average plot (default: 40)')
-    parser.add_argument('--num-stack', type=int, default=1, help='number of frames to stack (default: 1; state observations are not stacked here)')
+    parser.add_argument('--num-stack', type=int, default=1, help='number of frames to stack (default: 1)')
     parser.add_argument('-joints', '--action-joints', action='store_true', default=False, help='set actions to the joints of the arm directly')
     parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 hyper-parameters as name:value pairs')
     parser.add_argument('--log-dir', default='/tmp/gym/', type=str)
@@ -48,7 +48,7 @@ def main(argv=None):
     # sanity checks of the reference (train.py:221-224,265-266)
     assert args.episode_window >= 1, "Error: --episode_window cannot be less than 1"
     assert args.num_timesteps >= 1, "Error: --num-timesteps cannot be less than 1"
-    assert args.num_stack == 1, "Error: --num-stack > 1 is for image observations, which this simulator does not render"
+    assert args.num_stack >= 1, "Error: --num-stack cannot be less than 1"
     assert args.action_repeat >= 1, "Error: --action-repeat cannot be less than 1"
     if args.action_joints and not args.continuous_actions:
         raise ValueError("The joints action space is continuous only: use '-joints' together with '-c' (kuka_button_gym_env.py:149-161)")
@@ -73,12 +73,12 @@ def main(argv=None):
                 dist.init_process_group("nccl", device_id=torch.device("cuda", device))
         try:
             return train(args.env, args.num_cpu, num_timesteps, seed=args.seed, env_kwargs=env_kwargs, log_dir=log_dir, device=device,
-                         hyperparams=hyperparams, episode_window=args.episode_window)
+                         hyperparams=hyperparams, episode_window=args.episode_window, num_stack=args.num_stack)
         finally:
             if world > 1 and dist.is_initialized():
                 dist.destroy_process_group()
     from rl_baselines.random_agent import train
-    return train(args.env, args.num_cpu, num_timesteps, seed=args.seed, env_kwargs=env_kwargs)
+    return train(args.env, args.num_cpu, num_timesteps, seed=args.seed, env_kwargs=env_kwargs, num_stack=args.num_stack)
 
 
 if __name__ == '__main__':

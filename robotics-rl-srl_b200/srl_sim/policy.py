@@ -1,7 +1,7 @@
 """
-ctypes binding of ``include/srl_policy.h``: the two per-step helpers of a GPU-resident PPO2 rollout that live in the same
+ctypes binding of ``include/srl_policy.h``: the per-step helpers of a GPU-resident PPO2 rollout that live in the same
 sm_90a library as the simulator -- the policy step (both 64-64 towers, sample, log-probability, value, rollout-buffer writes
-in ONE launch) and the VecNormalize observation filter (ONE launch).  With ``srl_sim_step`` a captured rollout is then three
+in ONE launch) and the VecNormalize observation filter (ONE launch; with ``--num-stack k`` the frame stack step and the filter share it).  With ``srl_sim_step`` a captured rollout is then three
 launches per env step instead of ~60 small torch kernels around the simulator's.
 
 Reference pieces replaced: stable-baselines' ``PPO2`` runner ``model.step(obs)`` with ``MlpPolicy`` (selected by
@@ -11,8 +11,8 @@ There is no CPU fallback here either: :class:`FusedPolicy` needs the CUDA librar
 import ctypes
 from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64, c_void_p
 
-HIDDEN, MAX_OBS, MAX_OUT = 64, 8, 8
-POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae"]
+HIDDEN, MAX_OBS, MAX_OUT = 64, 32, 8     # observation widths 1..8 and 9..32 (stacked states) run separate kernel instantiations
+POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae"]
 
 
 class SrlMlpPolicy(Structure):
@@ -35,6 +35,8 @@ def bind(cdll):
     cdll.srl_policy_act.argtypes = [POINTER(SrlMlpPolicy), c_int, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     cdll.srl_obs_filter.restype = c_int
     cdll.srl_obs_filter.argtypes = [c_int, c_int, c_void_p, c_void_p, c_int, c_float, c_float, c_void_p, c_void_p]
+    cdll.srl_obs_stack_filter.restype = c_int
+    cdll.srl_obs_stack_filter.argtypes = [c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float, c_void_p, c_void_p]
     cdll.srl_ppo2_workspace_bytes.restype = c_size_t
     cdll.srl_ppo2_workspace_bytes.argtypes = [c_int, c_int, c_int, c_int]
     cdll.srl_ppo2_grad.restype = c_int
@@ -104,6 +106,17 @@ class FusedPolicy(object):
         rc = self._lib.srl_obs_filter(int(n), self.obs_dim, obs_raw.data_ptr(), self.filter_state.data_ptr(), int(bool(update)),
                                       self.clip, self.eps, obs_norm_out.data_ptr(), stream)
         self._library.check(rc, "srl_obs_filter")
+
+    def stack_filter(self, n, obs_raw, done, stack, obs_norm_out, update=True, stream=None):
+        """``srl_obs_stack_filter``: VecFrameStack + VecNormalize in one launch.  ``obs_raw`` float32 [n, D] with ``obs_dim`` a multiple k of D,
+        ``done`` uint8 [n] (None: a reset, every row starts from zeros), ``stack`` float32 [n, k D] advanced in place, ``obs_norm_out``
+        float32 [n, k D]; the filter state is this object's (2 k D + 1 doubles)."""
+        D = int(obs_raw.shape[-1])
+        if D < 1 or self.obs_dim % D:
+            raise ValueError("stack_filter: the policy width %d is not a multiple of the observation width %d" % (self.obs_dim, D))
+        rc = self._lib.srl_obs_stack_filter(int(n), D, self.obs_dim // D, obs_raw.data_ptr(), None if done is None else done.data_ptr(), stack.data_ptr(),
+                                            self.filter_state.data_ptr(), int(bool(update)), self.clip, self.eps, obs_norm_out.data_ptr(), stream)
+        self._library.check(rc, "srl_obs_stack_filter")
 
 
 class FusedPPO2Grad(object):
