@@ -116,8 +116,20 @@ enum srl_state_field {
                                  xyz w, body type (0 duck_vhacd, 1 lego, 2 cube_small, 3 sphere_small), present (0/1); slots 0-9
                                  are the 10 placements of reset() (absent inside the square around the button), slot 10 the
                                  kicked sphere; all zero without srl_sim_set_distractors                       */
-    SRL_F_DISTRACTOR_TOUCH = 14 /* i32[N,2] (read-only) bit k set: distractor slot k touched another body / the arm since its
+    SRL_F_DISTRACTOR_TOUCH = 14, /* i32[N,2] (read-only) bit k set: distractor slot k touched another body / the arm since its
                                  placement                                                                     */
+    /* Test hooks of the CUDA library's distractor bodies (copies of device buffers in their own float32 layout; not for
+     * applications, and not in the CPU oracle, which refuses them like every field it does not know): */
+    SRL_F_DISTRACTOR_RECORDS = 15, /* f32[N,11,16] the full body records (csrc/distractor_core.h, DC_B_*): position, quaternion
+                                 xyz w, v, w, type, present, 2 unused words.  Settable, so that a test can start the bodies from a
+                                 crafted configuration: every value finite, present 0 or 1, type 0-3, unit quaternion (1e-4), else the
+                                 call is refused.  The touch masks are left as they are.                       */
+    SRL_F_DISTRACTOR_TRACE_LEN = 16, /* i32[N,1] (read-only) micro-steps the last reset / step / rollout launch recorded per env */
+    SRL_F_DISTRACTOR_TRACE = 17, /* f32[N,L,16] (read-only) the first L records of that launch's trace per env, L = bytes / (64 N)
+                                 at most the launch's capacity T (action_repeat + 5) (5 for a reset): joint angles q[0-11], glider q,
+                                 button base x, y, and the tag word (bits of an int32: tag | episode << 4, csrc/kuka_state.cuh)  */
+    SRL_F_DISTRACTOR_SETTLE = 18 /* f32[500,16] (read-only, not per env) the arm's settle trajectory the bodies are settled against,
+                                 same record layout                                                            */
 };
 
 int srl_sim_abi_version(void);

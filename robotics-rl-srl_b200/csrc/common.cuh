@@ -128,5 +128,6 @@ int dist_alloc(srl_sim* s, const void* blob, size_t bytes, float4** settle);   /
 int dist_trace(srl_sim* s, size_t steps, cudaStream_t st, float4** trace, int** trace_len);   // trace buffers for <= `steps` micro-steps per env
 int dist_advance(srl_sim* s, const double* draws, cudaStream_t st);   // distractor_kernel through the micro-steps of the last traced launch
 void dist_free(srl_sim* s);
-int dist_get_state(srl_sim* s, int field, void* dst, size_t bytes);   // SRL_F_DISTRACTORS, SRL_F_DISTRACTOR_TOUCH
+int dist_get_state(srl_sim* s, int field, void* dst, size_t bytes);   // SRL_F_DISTRACTORS, SRL_F_DISTRACTOR_TOUCH and the SRL_F_DISTRACTOR_* test hooks
+int dist_set_state(srl_sim* s, const void* src, size_t bytes);   // SRL_F_DISTRACTOR_RECORDS
 const float* dist_render_bodies(const srl_sim* s, SrlBodyLooks* looks);   // [N][DC_NBODY][DC_B_WORDS] body poses + drawing table; nullptr: no bodies

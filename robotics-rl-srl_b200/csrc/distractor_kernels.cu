@@ -226,22 +226,73 @@ const float* dist_render_bodies(const srl_sim* s, SrlBodyLooks* looks) {
     return s->dist->body;
 }
 
-// SRL_F_DISTRACTORS and SRL_F_DISTRACTOR_TOUCH of kuka_get_state: zeros for a handle without bodies
+// SRL_F_DISTRACTORS and SRL_F_DISTRACTOR_TOUCH of kuka_get_state: zeros for a handle without bodies.  The test hooks (SRL_F_DISTRACTOR_RECORDS,
+// _TRACE_LEN, _TRACE, _SETTLE) are plain copies of the device buffers and need the bodies.
 int dist_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
     const size_t N = (size_t)s->n;
-    const bool touch = field == SRL_F_DISTRACTOR_TOUCH;
-    if (bytes != (touch ? N * 2 * sizeof(uint32_t) : N * DC_NBODY * 9 * sizeof(double))) { srl_set_error("get_state: size mismatch"); return 1; }
-    memset(dst, 0, bytes);
     const DistDev* g = s->dist;
-    if (!g) return 0;
-    if (touch) { SRL_CUDA_OK(cudaMemcpy(dst, g->touch, bytes, cudaMemcpyDeviceToHost)); return 0; }
-    std::vector<float> h(N * DC_NBODY * DC_B_WORDS);
-    SRL_CUDA_OK(cudaMemcpy(h.data(), g->body, h.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < N * DC_NBODY; ++i) {
-        const float* b = h.data() + i * DC_B_WORDS;
-        double* o = (double*)dst + i * 9;
-        for (int a = 0; a < 7; ++a) o[a] = b[DC_B_P + a];   // position, quaternion (x y z w)
-        o[7] = b[DC_B_TYPE]; o[8] = b[DC_B_PRESENT];
+    if (field == SRL_F_DISTRACTORS || field == SRL_F_DISTRACTOR_TOUCH) {
+        const bool touch = field == SRL_F_DISTRACTOR_TOUCH;
+        if (bytes != (touch ? N * 2 * sizeof(uint32_t) : N * DC_NBODY * 9 * sizeof(double))) { srl_set_error("get_state: size mismatch"); return 1; }
+        memset(dst, 0, bytes);
+        if (!g) return 0;
+        if (touch) { SRL_CUDA_OK(cudaMemcpy(dst, g->touch, bytes, cudaMemcpyDeviceToHost)); return 0; }
+        std::vector<float> h(N * DC_NBODY * DC_B_WORDS);
+        SRL_CUDA_OK(cudaMemcpy(h.data(), g->body, h.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < N * DC_NBODY; ++i) {
+            const float* b = h.data() + i * DC_B_WORDS;
+            double* o = (double*)dst + i * 9;
+            for (int a = 0; a < 7; ++a) o[a] = b[DC_B_P + a];   // position, quaternion (x y z w)
+            o[7] = b[DC_B_TYPE]; o[8] = b[DC_B_PRESENT];
+        }
+        return 0;
     }
+    if (!g) { srl_set_error("get_state: field %d needs srl_sim_set_distractors", field); return 1; }
+    switch (field) {
+    case SRL_F_DISTRACTOR_RECORDS:
+        if (bytes != N * DC_NBODY * DC_B_WORDS * sizeof(float)) { srl_set_error("get_state: size mismatch"); return 1; }
+        SRL_CUDA_OK(cudaMemcpy(dst, g->body, bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    case SRL_F_DISTRACTOR_TRACE_LEN:
+        if (bytes != N * sizeof(int)) { srl_set_error("get_state: size mismatch"); return 1; }
+        SRL_CUDA_OK(cudaMemcpy(dst, g->trace_len, bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    case SRL_F_DISTRACTOR_SETTLE:
+        if (bytes != 500 * 4 * sizeof(float4)) { srl_set_error("get_state: size mismatch"); return 1; }
+        SRL_CUDA_OK(cudaMemcpy(dst, g->settle, bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    case SRL_F_DISTRACTOR_TRACE: {
+        const size_t L = bytes / (N * 4 * sizeof(float4));
+        if (L == 0 || L > g->cap || bytes != L * N * 4 * sizeof(float4)) { srl_set_error("get_state: the trace holds %zu records per env", g->cap); return 1; }
+        std::vector<float4> h(L * 4 * N);     // [micro-step][4][N] on the device -> [N][micro-step][4]
+        SRL_CUDA_OK(cudaMemcpy(h.data(), g->trace, h.size() * sizeof(float4), cudaMemcpyDeviceToHost));
+        float4* o = (float4*)dst;
+        for (size_t i = 0; i < N; ++i)
+            for (size_t m = 0; m < L; ++m)
+                for (size_t r = 0; r < 4; ++r) o[(i * L + m) * 4 + r] = h[(m * 4 + r) * N + i];
+        return 0;
+    }
+    default:
+        srl_set_error("get_state: unknown field %d", field);
+        return 1;
+    }
+}
+
+// SRL_F_DISTRACTOR_RECORDS of kuka_set_state (test hook): valid records only
+int dist_set_state(srl_sim* s, const void* src, size_t bytes) {
+    const size_t N = (size_t)s->n;
+    DistDev* g = s->dist;
+    if (!g) { srl_set_error("set_state: the distractor records need srl_sim_set_distractors"); return 1; }
+    if (bytes != N * DC_NBODY * DC_B_WORDS * sizeof(float)) { srl_set_error("set_state: size mismatch"); return 1; }
+    for (size_t i = 0; i < N * DC_NBODY; ++i) {
+        const float* b = (const float*)src + i * DC_B_WORDS;
+        for (int a = 0; a < DC_B_WORDS; ++a)
+            if (!isfinite(b[a])) { srl_set_error("set_state: distractor record %zu has a non-finite value", i); return 1; }
+        if (b[DC_B_PRESENT] != 0.f && b[DC_B_PRESENT] != 1.f) { srl_set_error("set_state: distractor record %zu: present must be 0 or 1", i); return 1; }
+        if (!(b[DC_B_TYPE] == 0.f || b[DC_B_TYPE] == 1.f || b[DC_B_TYPE] == 2.f || b[DC_B_TYPE] == 3.f)) { srl_set_error("set_state: distractor record %zu: type must be 0, 1, 2 or 3", i); return 1; }
+        const double qq = (double)b[DC_B_Q] * b[DC_B_Q] + (double)b[DC_B_Q + 1] * b[DC_B_Q + 1] + (double)b[DC_B_Q + 2] * b[DC_B_Q + 2] + (double)b[DC_B_Q + 3] * b[DC_B_Q + 3];
+        if (fabs(sqrt(qq) - 1.0) > 1e-4) { srl_set_error("set_state: distractor record %zu: the quaternion is not of unit length", i); return 1; }
+    }
+    SRL_CUDA_OK(cudaMemcpy(g->body, src, bytes, cudaMemcpyHostToDevice));
     return 0;
 }

@@ -32,6 +32,28 @@ int dref_run(const double* blob, size_t bytes, const double* scene, double dt, i
     return 0;
 }
 
+// dref_run with a scene that changes per micro-step, as the kernel replays a trace: arm = f64[n_steps][narm][4], disc (nullable) =
+// f64[n_steps][2] the disc's absolute z range, kicks (nullable) = f64[n_steps][3] impulses, applied where kick_on[s] != 0.
+// touch (nullable): u32[2], OR-ed into.
+int dref_run_steps(const double* blob, size_t bytes, const double* scene, double dt, int iters, double margin, double* B, const double* arm, int narm,
+                   int n_steps, const double* disc, const double* kicks, const uint8_t* kick_on, double* traj, uint32_t* touch) {
+    if (dc_blob_error(blob, bytes)) return 1;
+    DcAssets<double> A; dc_assets_from_blob(blob, A);
+    DcScene<double> S; scene_from(scene, dt, iters, margin, S);
+    std::vector<DcRow<double>> rows(3 * DC_MAXC);
+    DcTouch t = {0u, 0u};
+    for (int s = 0; s < n_steps; ++s) {
+        if (disc) { S.disc0 = disc[2 * s]; S.disc1 = disc[2 * s + 1]; }
+        dc_step(A, S, B, arm + (size_t)s * narm * 4, narm, (kicks && kick_on[s]) ? kicks + 3 * s : nullptr, rows.data(), &t);
+        if (traj) memcpy(traj + (size_t)s * DC_NBODY * DC_B_WORDS, B, sizeof(double) * DC_NBODY * DC_B_WORDS);
+    }
+    if (touch) { touch[0] |= t.body; touch[1] |= t.arm; }
+    return 0;
+}
+
+// the islands of an adjacency (adj[k] bit m > k: bodies k and m are within the margin): root[k] = lowest slot of body k's island
+void dref_island_roots(const uint32_t* adj, int* root) { dc_island_roots(adj, root); }
+
 // reset()'s placement rule: B from 20 placement values (x0, y0, ..., x9, y9), 10 types and the button position
 void dref_place(const double* xy, const int* type, double btn_x, double btn_y, double* B) { dc_place(B, xy, type, btn_x, btn_y); }
 

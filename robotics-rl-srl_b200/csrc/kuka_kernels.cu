@@ -963,6 +963,7 @@ int kuka_get_state(srl_sim* s, int field, void* dst, size_t bytes) {
     }
 #endif
     case SRL_F_DISTRACTORS: case SRL_F_DISTRACTOR_TOUCH:
+    case SRL_F_DISTRACTOR_RECORDS: case SRL_F_DISTRACTOR_TRACE_LEN: case SRL_F_DISTRACTOR_TRACE: case SRL_F_DISTRACTOR_SETTLE:
         return dist_get_state(s, field, dst, bytes);
     case SRL_F_NEXT_RECORD: {
         if (!need(3, 4)) return 1;
@@ -1039,6 +1040,8 @@ int kuka_set_state(srl_sim* s, int field, const void* src, size_t bytes) {
         SRL_CUDA_OK(cudaMemcpy(d->cnt, ia.data(), N * sizeof(int4), cudaMemcpyHostToDevice));
         return 0;
     }
+    case SRL_F_DISTRACTOR_RECORDS:
+        return dist_set_state(s, src, bytes);
     default:
         srl_set_error("set_state: field %d not settable", field);
         return 1;

@@ -32,7 +32,8 @@ ENV_KINDS = {
 
 # enum srl_state_field
 F_ROBOT_POS, F_TARGET_POS, F_STEP_COUNTER, F_JOINT_POS, F_JOINT_VEL, F_EE_CMD, F_EE_POS, \
-    F_BUTTON_GLIDER, F_COUNTERS, F_EPISODE_STATS, F_BUTTON_BASE, F_TWO_BUTTON, F_NEXT_RECORD, F_DISTRACTORS, F_DISTRACTOR_TOUCH = range(15)
+    F_BUTTON_GLIDER, F_COUNTERS, F_EPISODE_STATS, F_BUTTON_BASE, F_TWO_BUTTON, F_NEXT_RECORD, F_DISTRACTORS, F_DISTRACTOR_TOUCH, \
+    F_DISTRACTOR_RECORDS, F_DISTRACTOR_TRACE_LEN, F_DISTRACTOR_TRACE, F_DISTRACTOR_SETTLE = range(19)
 
 _FIELD_SPEC = {
     F_ROBOT_POS: (np.float64, 3), F_TARGET_POS: (np.float64, 3), F_STEP_COUNTER: (np.int32, 1),
@@ -40,6 +41,7 @@ _FIELD_SPEC = {
     F_EE_POS: (np.float64, 3), F_BUTTON_GLIDER: (np.float64, 2), F_COUNTERS: (np.int32, 4),
     F_EPISODE_STATS: (np.float64, 2), F_BUTTON_BASE: (np.float64, 3), F_TWO_BUTTON: (np.float64, 8), F_NEXT_RECORD: (np.int32, 3),
     F_DISTRACTORS: (np.float64, 11 * 9), F_DISTRACTOR_TOUCH: (np.int32, 2),
+    F_DISTRACTOR_RECORDS: (np.float32, 11 * 16), F_DISTRACTOR_TRACE_LEN: (np.int32, 1),   # test hooks of the CUDA library
 }
 
 MOBILE_RESET_DRAWS = 6
@@ -264,6 +266,18 @@ class Sim(object):
         arr = np.ascontiguousarray(np.asarray(values, dtype=dtype).reshape(self.num_envs, width))
         rc = self._lib.srl_sim_set_state(self.handle, field, arr.ctypes.data, arr.nbytes)
         self.library.check(rc, "srl_sim_set_state")
+
+    def distractor_trace(self):
+        """Test hook of the CUDA library: what the bodies replayed in the last launch.  Returns (trace_len i32[N], trace f32[N, L, 16] with
+        L = max(trace_len), the tag words as i32[N, L], the handle's settle trajectory f32[500, 16])."""
+        length = self.get_state(F_DISTRACTOR_TRACE_LEN).reshape(-1)
+        trace = np.zeros((self.num_envs, max(int(length.max()), 1), 16), np.float32)
+        rc = self._lib.srl_sim_get_state(self.handle, F_DISTRACTOR_TRACE, trace.ctypes.data, trace.nbytes)
+        self.library.check(rc, "srl_sim_get_state")
+        settle = np.zeros((500, 16), np.float32)
+        rc = self._lib.srl_sim_get_state(self.handle, F_DISTRACTOR_SETTLE, settle.ctypes.data, settle.nbytes)
+        self.library.check(rc, "srl_sim_get_state")
+        return length, trace, np.ascontiguousarray(trace[:, :, 15]).view(np.int32), settle
 
     @property
     def launch_count(self):

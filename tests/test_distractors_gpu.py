@@ -187,11 +187,9 @@ def test_bench_size_outputs_identical_and_sphere_kicked(cuda):
         outs.append([cuda.to_host(x).copy() for x in o])
         if bodies:
             after = _bodies(s)[:, 10, 0:3]
-            first_done = np.argmax(outs[1][2], axis=0)
             no_reset = ~outs[1][2].any(axis=0)
             moved = after[no_reset] - before[no_reset]
             print("envs without a reset: %d, sphere moved +x in %d, +y in %d" % (no_reset.sum(), (moved[:, 0] > 0).sum(), (moved[:, 1] > 0).sum()))
-            del first_done
     for a, b in zip(outs[0], outs[1]):
         assert a.tobytes() == b.tobytes()
     # the kick at step 10 sends the sphere towards +x, +y; over the remaining 118 steps some run into an object, the button or the arm
