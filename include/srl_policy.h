@@ -12,6 +12,9 @@
  *                      by rl_baselines/utils.py:224-227: running mean / variance update + normalisation
  *   srl_obs_stack_filter <- `VecFrameStack(envs, num_stack)` -> `VecNormalize` (rl_baselines/utils.py:222-227): the frame stack
  *                      step and the filter of the stacked rows in one launch
+ *   srl_a2c_grad    <- the loss + `tf.gradients` of stable-baselines 2.5 `A2C.setup_model`, run once per update by `A2C._train_step`
+ *                      (chosen by rl_baselines/rl_algorithm/a2c.py)
+ *   srl_clip_rmsprop <- the same `_train_step`'s `tf.clip_by_global_norm` + `tf.train.RMSPropOptimizer` apply op
  *
  * Conventions are those of srl_sim.h: 0 on success, message from srl_sim_last_error(); all pointers are DEVICE pointers;
  * calls are asynchronous on `stream` and capturable into a CUDA graph (everything a launch reads that changes between
@@ -94,11 +97,39 @@ int srl_ppo2_grad(const srl_mlp_policy* policy, const srl_mlp_grads* grads, int 
                   const void* actions, const float* adv, const float* ret, const float* old_logp, const float* old_value,
                   float cliprange, float ent_coef, float vf_coef, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The gradient of stable-baselines 2.5's A2C loss over `rows` rows, written into `grads` like srl_ppo2_grad (same kernels and chunking, same
+ * deterministic CTA-order reduction; only the per-sample loss derivative differs):
+ *   ADV = ret - old_value (not normalised), pg_loss = mean(-ADV logp(a)), vf_loss = 0.5 mean((v - ret)^2),
+ *   loss = pg_loss - ent_coef * mean(entropy) + vf_coef * vf_loss.
+ * RECALLED, not checked against an installed stable-baselines (none can be installed here; re-pin these when one is): the 0.5 of vf_loss
+ * (`mse()` of stable_baselines/a2c/utils.py divides by 2), and that A2C clips neither the value nor the probability ratio.
+ *   idx : nullable i64[rows] row indices (NULL: rows 0 .. rows - 1); obs, actions, ret, old_value as for srl_ppo2_grad
+ *   workspace : at least srl_a2c_workspace_bytes(...) bytes (per-CTA partial gradients; no state between calls) */
+size_t srl_a2c_workspace_bytes(int obs_dim, int n_out, int discrete, int rows);   /* 0 for an unsupported shape */
+int srl_a2c_grad(const srl_mlp_policy* policy, const srl_mlp_grads* grads, int rows, const int64_t* idx, const float* obs, const void* actions,
+                 const float* ret, const float* old_value, float ent_coef, float vf_coef, void* workspace, size_t workspace_bytes, void* stream);
+
+/* One optimiser step of stable-baselines' A2C over every tensor of an MlpPolicy, in one launch:
+ *   tf.clip_by_global_norm(grads, max_grad_norm): norm = sqrt(sum of every squared gradient entry), scale = max_grad_norm / max(norm, max_grad_norm);
+ *     a NaN or infinite norm makes the scale NaN, so one non-finite gradient entry turns every parameter NaN (TF's behaviour);
+ *   tf.train.RMSPropOptimizer(lr, decay=alpha, epsilon, momentum=0) on g = scale * grad:
+ *     ms <- ms + (g^2 - ms) (1 - alpha);   param <- param - lr g / sqrt(ms + epsilon).
+ * RECALLED from TF 1.x, not checked against an installed TF: the `ms` slot starts at 1.0 (not 0; the caller initialises it), and epsilon sits
+ * inside the square root.  This is not torch.optim.RMSprop.
+ *   params, grads, ms : the tensors of the policy, its gradients and the RMSProp slot, each in the layout of srl_mlp_grads for this shape
+ *                       (logstd only for Box); params and ms are updated in place, grads are read
+ *   lr : f32[1] device scalar (a captured call follows a schedule that rewrites it)
+ * The squared norm is summed in float64 in a fixed order: two calls on the same inputs give the same bytes.  No host synchronisation. */
+int srl_clip_rmsprop(int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, const srl_mlp_grads* grads, const srl_mlp_grads* ms,
+                     const float* lr, float max_grad_norm, float alpha, float epsilon, void* stream);
+
 /* GAE(lambda) over one rollout (the backward recursion of stable-baselines' PPO2 runner): rew, value, done (1.0 where the episode ended at that
  * step), adv_out, ret_out are f32[n_steps, n_envs]; last_value f32[n_envs] is the value of the observation after the last step.
  *   delta_t = rew_t + gamma * V_{t+1} * (1 - done_t) - V_t;  adv_t = delta_t + gamma * lam * (1 - done_t) * adv_{t+1};  ret_t = adv_t + V_t
  * gamma and lam are doubles: the float32 recursion uses fl32(gamma) and fl32(gamma * lam), the coefficients a float32 array expression with
- * Python-float hyper-parameters uses (fl32(gamma) * fl32(lam) is another float for e.g. gamma = lam = 0.9). */
+ * Python-float hyper-parameters uses (fl32(gamma) * fl32(lam) is another float for e.g. gamma = lam = 0.9).
+ * With lam = 1, ret_t = rew_t + gamma (1 - done_t) ret_{t+1} from ret_{n_steps} = last_value: A2C's bootstrapped n-step returns
+ * (stable-baselines' `discount_with_dones` over the rewards followed by the last value). */
 int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, double gamma, double lam,
                  float* adv_out, float* ret_out, void* stream);
 

@@ -108,7 +108,7 @@ __device__ __forceinline__ float dot64(const float* row, const float* col) {
 
 struct SampleRegs { float x[MAXD], af[MAXO], adv, ret, olp, ov; int ai, valid; };
 
-template <bool LOAD_X>
+template <bool LOAD_X, bool A2C>
 __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs& r) {
     const int D = a.p.obs_dim, A = a.p.n_out;
     r.valid = s < a.mb;
@@ -127,7 +127,8 @@ __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs
             for (int k = 0; k < MAXO; ++k) if (k < A) r.af[k] = reinterpret_cast<const float*>(a.act)[g * A + k];
         }
     }
-    r.adv = r.valid ? a.adv[g] : 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = r.valid ? a.old_logp[g] : 0.f; r.ov = r.valid ? a.old_val[g] : 0.f;
+    if constexpr (A2C) { r.adv = 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = 0.f; r.ov = r.valid ? a.old_val[g] : 0.f; }   // advantage: ret - old_val
+    else { r.adv = r.valid ? a.adv[g] : 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = r.valid ? a.old_logp[g] : 0.f; r.ov = r.valid ? a.old_val[g] : 0.f; }
 }
 
 // The wide instantiation (MD = WIDE_D) differs from the narrow one (MD = MAXD) in three places, all to fit shared memory and registers:
@@ -148,7 +149,8 @@ __device__ __forceinline__ void load_row_part(const GradArgs& a, int s, int u, f
 
 template <int MD>
 __host__ __device__ constexpr int grad_w1_stride() { return MD == MAXD ? MAXD : MD + 1; }
-template <int MD>
+// A2C: the loss of srl_a2c_grad instead of PPO2's (stage 2 only; no advantage statistics, no clip ratio, no value clip)
+template <int MD, bool A2C>
 __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     constexpr bool WIDE = MD != MAXD;
     constexpr int W1S = grad_w1_stride<MD>(), XQ = MD / 4;     // XQ: observation columns per thread of the wide prefetch
@@ -188,7 +190,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     if (t < A) { b3p[t] = a.p.pi_b3[t]; lsd[t] = discrete ? 0.f : a.p.logstd[t]; }
     if (t == 0) b3v[0] = a.p.vf_b3[0];
     __shared__ float s_adv[2];
-    if (t < 32) {                  // mean and 1 / (std + 1e-8) (torch.std(): unbiased) from the partial sums, in a fixed order
+    if (!A2C && t < 32) {                  // mean and 1 / (std + 1e-8) (torch.std(): unbiased) from the partial sums, in a fixed order
         double s1 = a.stats[2 * t] + a.stats[2 * (t + 32)], s2 = a.stats[2 * t + 1] + a.stats[2 * (t + 32) + 1];
         for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
         if (t == 0) {
@@ -198,7 +200,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
         }
     }
     __syncthreads();
-    const float amean = s_adv[0], ainv = s_adv[1], inv_mb = 1.0f / (float)a.mb;
+    const float amean = A2C ? 0.f : s_adv[0], ainv = A2C ? 0.f : s_adv[1], inv_mb = 1.0f / (float)a.mb;
     // ---- gradient accumulators (registers; every entry of the flat gradient has exactly one owner thread) ----
     const int eg = t >> 4, og = t & 15;          // forward / delta tiles: samples 4 eg + e, units og + 16 k
     const bool own_pi = t < 128;                 // W2 gradient: threads 0..127 own the policy tower's 4 x 8 patches, 128..255 the value tower's
@@ -215,7 +217,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     const int nchunks = (a.mb + CH - 1) / CH;
     SampleRegs cur;
     float xr[XQ];                                // wide: this thread's columns t % 4 + 4 j of sample t / 4 of the next chunk
-    if (t < CH) load_sample<!WIDE>(a, blockIdx.x * CH + t, cur);
+    if (t < CH) load_sample<!WIDE, A2C>(a, blockIdx.x * CH + t, cur);
     if constexpr (WIDE) load_row_part<XQ>(a, blockIdx.x * CH + (t >> 2), t & 3, xr);
     __syncthreads();
     for (int c = blockIdx.x; c < nchunks; c += gridDim.x) {
@@ -229,7 +231,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
             for (int k = 0; k < MAXO; ++k) saf[t * MAXO + k] = cur.af[k];
             ssc[t * 4] = cur.adv; ssc[t * 4 + 1] = cur.ret; ssc[t * 4 + 2] = cur.olp; ssc[t * 4 + 3] = cur.ov;
             sai[t * 2] = cur.ai; sai[t * 2 + 1] = cur.valid;
-            load_sample<!WIDE>(a, (c + gridDim.x) * CH + t, cur);
+            load_sample<!WIDE, A2C>(a, (c + gridDim.x) * CH + t, cur);
         }
         if constexpr (WIDE) {
 #pragma unroll
@@ -321,11 +323,16 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
                         p[k] = u;                      // (a - mu) / sigma, reused below
                     }
                 }
-                const float ratio = expf(logp - olp);
-                const float rc = fminf(fmaxf(ratio, 1.0f - c), 1.0f + c);
-                const float unclipped = -An * ratio, clipped = -An * rc;
-                const float dr = (rc == ratio || unclipped > clipped) ? -An : 0.f;      // max(): the live branch (a tie inside the clip range sums to the same)
-                const float dlogp = dr * ratio * inv_mb;
+                float dlogp;
+                if constexpr (A2C) {
+                    dlogp = -(R - ov) * inv_mb;                                         // pg_loss = mean(-(R - V) logp)
+                } else {
+                    const float ratio = expf(logp - olp);
+                    const float rc = fminf(fmaxf(ratio, 1.0f - c), 1.0f + c);
+                    const float unclipped = -An * ratio, clipped = -An * rc;
+                    const float dr = (rc == ratio || unclipped > clipped) ? -An : 0.f;  // max(): the live branch (a tie inside the clip range sums to the same)
+                    dlogp = dr * ratio * inv_mb;
+                }
                 if (discrete) {
                     const int ai = sai[n * 2];
                     const float ec = a.ent_coef * inv_mb;
@@ -339,10 +346,14 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
                         gl[k] = dlogp * (p[k] * p[k] - 1.0f) - a.ent_coef * inv_mb;     // d logp / d logstd; entropy = sum(logstd) + const
                     }
                 }
-                const float dv = v - ov, dvc = fminf(fmaxf(dv, -c), c);
-                const float e1 = v - R, e2 = (ov + dvc) - R;
-                const float l1 = e1 * e1, l2 = e2 * e2;
-                gv = (dvc == dv || l1 > l2) ? e1 : (l1 == l2 ? 0.5f * e1 : 0.f);
+                if constexpr (A2C) {
+                    gv = v - R;                                                         // vf_loss = 0.5 mean((v - R)^2)
+                } else {
+                    const float dv = v - ov, dvc = fminf(fmaxf(dv, -c), c);
+                    const float e1 = v - R, e2 = (ov + dvc) - R;
+                    const float l1 = e1 * e1, l2 = e2 * e2;
+                    gv = (dvc == dv || l1 > l2) ? e1 : (l1 == l2 ? 0.5f * e1 : 0.f);
+                }
                 gv *= a.vf_coef * inv_mb;
             }
 #pragma unroll
@@ -490,8 +501,10 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     if (!discrete && t >= 16 && t < 16 + A) out[seg.ls + (t - 16)] = gls;
 }
 
-__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD>(a); }
-__global__ void __launch_bounds__(NT, 1) ppo2_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D>(a); }
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, false>(a); }
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, false>(a); }
+__global__ void __launch_bounds__(NT, 1) a2c_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, true>(a); }
+__global__ void __launch_bounds__(NT, 1) a2c_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, true>(a); }
 
 // GAE(lambda) of one rollout, the reference's backward recursion (stable-baselines PPO2 runner): one thread per env, T sequential steps,
 // eight steps' loads in flight.  Separate roundings (no FMA contraction): the same bits as the torch recursion of rl_baselines/ppo2.py.
@@ -543,6 +556,50 @@ __global__ void ppo2_reduce_kernel(const __grid_constant__ ReduceArgs r) {
     dst[off] = s;
 }
 
+// TF1 `clip_by_global_norm` then `RMSPropOptimizer(momentum=0)` over every tensor of the policy (include/srl_policy.h: srl_clip_rmsprop).
+// One CTA: 9-13 k parameters are one pass of 1024 threads; the squared norm is summed in float64 in a fixed order (thread-strided, then a
+// shuffle tree, then the 32 warps in order), so two calls give the same bytes.  The update keeps TF's expression order with separate
+// float32 roundings (no FMA contraction), the order rl_baselines/a2c.py's torch restatement evaluates.
+constexpr int OPT_NT = 1024;
+struct OptArgs { srl_mlp_grads p, g, ms; Seg seg; const float* lr; float max_norm, alpha, eps; };
+
+__device__ __forceinline__ float* seg_elem(const srl_mlp_grads& t, const Seg& q, int e) {
+    if (e < q.pb1) return t.pi_w1 + (e - q.pw1); if (e < q.pw2) return t.pi_b1 + (e - q.pb1);
+    if (e < q.pb2) return t.pi_w2 + (e - q.pw2); if (e < q.pw3) return t.pi_b2 + (e - q.pb2);
+    if (e < q.pb3) return t.pi_w3 + (e - q.pw3); if (e < q.vw1) return t.pi_b3 + (e - q.pb3);
+    if (e < q.vb1) return t.vf_w1 + (e - q.vw1); if (e < q.vw2) return t.vf_b1 + (e - q.vb1);
+    if (e < q.vb2) return t.vf_w2 + (e - q.vw2); if (e < q.vw3) return t.vf_b2 + (e - q.vb2);
+    if (e < q.vb3) return t.vf_w3 + (e - q.vw3); if (e < q.ls) return t.vf_b3 + (e - q.vb3);
+    return t.logstd + (e - q.ls);
+}
+
+__global__ void __launch_bounds__(OPT_NT, 1) clip_rmsprop_kernel(const __grid_constant__ OptArgs o) {
+    __shared__ double red[OPT_NT / 32];
+    __shared__ float s_scale;
+    const int t = threadIdx.x;
+    double s = 0.0;
+    for (int e = t; e < o.seg.P; e += OPT_NT) { const double g = (double)*seg_elem(o.g, o.seg, e); s = fma(g, g, s); }
+    for (int k = 16; k > 0; k >>= 1) s += __shfl_xor_sync(0xffffffffu, s, k);
+    if ((t & 31) == 0) red[t >> 5] = s;
+    __syncthreads();
+    if (t == 0) {
+        double tot = 0.0;
+        for (int w = 0; w < OPT_NT / 32; ++w) tot += red[w];
+        const double norm = sqrt(tot);      // + (norm - norm): NaN for a non-finite norm, so that every tensor becomes NaN, as in TF
+        s_scale = (float)((double)o.max_norm / fmax(norm, (double)o.max_norm) + (norm - norm));     // scale = max_norm / max(norm, max_norm)
+    }
+    __syncthreads();
+    const float scale = s_scale, lr = *o.lr, rho1 = __fsub_rn(1.0f, o.alpha);
+    for (int e = t; e < o.seg.P; e += OPT_NT) {
+        const float g = __fmul_rn(*seg_elem(o.g, o.seg, e), scale);
+        float* msp = seg_elem(o.ms, o.seg, e);
+        float* wp = seg_elem(o.p, o.seg, e);
+        const float ms = __fadd_rn(*msp, __fmul_rn(__fsub_rn(__fmul_rn(g, g), *msp), rho1));        // ms += (g^2 - ms) (1 - alpha)
+        *msp = ms;
+        *wp = __fsub_rn(*wp, __fdiv_rn(__fmul_rn(g, lr), __fsqrt_rn(__fadd_rn(ms, o.eps))));          // w -= g lr / sqrt(ms + eps)
+    }
+}
+
 template <int MD>
 constexpr size_t grad_smem_bytes() {
     return sizeof(float) * (size_t)(4 * H * WS + MAXO * WS + WS + (MD == MAXD ? 8 : 6) * CH * WS + 2 * H * grad_w1_stride<MD>() + 4 * H + MAXO + 4 + MAXO +
@@ -558,6 +615,42 @@ int grid_ctas(int mb) {
     if (!sms[dev]) { if (cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return 0; }
     const int chunks = (mb + CH - 1) / CH;
     return chunks < sms[dev] ? chunks : sms[dev];
+}
+
+// the checks srl_ppo2_grad and srl_a2c_grad share (`who` prefixes the message); the grid size, or 0 after setting the error
+int grad_args_ok(const char* who, const srl_mlp_policy* p, const srl_mlp_grads* grads, int minibatch) {
+    if (p->struct_size != sizeof(srl_mlp_policy) || grads->struct_size != sizeof(srl_mlp_grads)) { srl_set_error("%s: struct size mismatch", who); return 0; }
+    if (p->obs_dim < 1 || p->obs_dim > WIDE_D || p->n_out < 1 || p->n_out > MAXO || (p->discrete && p->n_out < 2) || minibatch < 1) {
+        srl_set_error("%s: unsupported shape obs_dim=%d n_out=%d minibatch=%d (obs_dim 1..%d, n_out 1..%d)", who, p->obs_dim, p->n_out, minibatch,
+                      WIDE_D, MAXO); return 0;
+    }
+    if (!p->pi_w1 || !p->pi_b1 || !p->pi_w2 || !p->pi_b2 || !p->pi_w3 || !p->pi_b3 || !p->vf_w1 || !p->vf_b1 || !p->vf_w2 || !p->vf_b2 || !p->vf_w3 ||
+        !p->vf_b3 || (!p->discrete && !p->logstd)) { srl_set_error("%s: null weight pointer", who); return 0; }
+    if (!grads->pi_w1 || !grads->pi_b1 || !grads->pi_w2 || !grads->pi_b2 || !grads->pi_w3 || !grads->pi_b3 || !grads->vf_w1 || !grads->vf_b1 || !grads->vf_w2 ||
+        !grads->vf_b2 || !grads->vf_w3 || !grads->vf_b3 || (!p->discrete && !grads->logstd)) { srl_set_error("%s: null gradient pointer", who); return 0; }
+    const int ctas = grid_ctas(minibatch);
+    if (ctas <= 0) srl_set_error("%s: no CUDA device", who);
+    return ctas;
+}
+
+// the gradient kernel of the row width (narrow or wide instantiation), then the CTA-order reduction into the gradient tensors
+template <void (*NARROW)(GradArgs), void (*WIDE)(GradArgs)>
+int launch_grad(const GradArgs& a, const srl_mlp_grads* grads, int ctas, cudaStream_t st) {
+    if (a.p.obs_dim <= MAXD) {
+        constexpr size_t smem = grad_smem_bytes<MAXD>();
+        SRL_CUDA_OK(srl_smem_opt_in<NARROW>(smem));
+        NARROW<<<ctas, NT, smem, st>>>(a);
+    } else {
+        constexpr size_t smem = grad_smem_bytes<WIDE_D>();
+        SRL_CUDA_OK(srl_smem_opt_in<WIDE>(smem));
+        WIDE<<<ctas, NT, smem, st>>>(a);
+    }
+    SRL_CUDA_OK(cudaGetLastError());
+    ReduceArgs r;
+    r.g = *grads; r.seg = make_seg(a.p.obs_dim, a.p.n_out, a.p.discrete); r.nparts = ctas; r.partial = a.partial;
+    ppo2_reduce_kernel<<<(r.seg.P + 255) / 256, 256, 0, st>>>(r);
+    SRL_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 }  // namespace
@@ -579,17 +672,8 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
                   const float* adv, const float* ret, const float* old_logp, const float* old_value, float cliprange, float ent_coef, float vf_coef,
                   void* workspace, size_t workspace_bytes, void* stream) {
     if (!p || !grads || !obs || !actions || !adv || !ret || !old_logp || !old_value || !workspace) { srl_set_error("ppo2_grad: null argument"); return 1; }
-    if (p->struct_size != sizeof(srl_mlp_policy) || grads->struct_size != sizeof(srl_mlp_grads)) { srl_set_error("ppo2_grad: struct size mismatch"); return 1; }
-    if (p->obs_dim < 1 || p->obs_dim > WIDE_D || p->n_out < 1 || p->n_out > MAXO || (p->discrete && p->n_out < 2) || minibatch < 1) {
-        srl_set_error("ppo2_grad: unsupported shape obs_dim=%d n_out=%d minibatch=%d (obs_dim 1..%d, n_out 1..%d)", p->obs_dim, p->n_out, minibatch,
-                      WIDE_D, MAXO); return 1;
-    }
-    if (!p->pi_w1 || !p->pi_b1 || !p->pi_w2 || !p->pi_b2 || !p->pi_w3 || !p->pi_b3 || !p->vf_w1 || !p->vf_b1 || !p->vf_w2 || !p->vf_b2 || !p->vf_w3 ||
-        !p->vf_b3 || (!p->discrete && !p->logstd)) { srl_set_error("ppo2_grad: null weight pointer"); return 1; }
-    if (!grads->pi_w1 || !grads->pi_b1 || !grads->pi_w2 || !grads->pi_b2 || !grads->pi_w3 || !grads->pi_b3 || !grads->vf_w1 || !grads->vf_b1 || !grads->vf_w2 ||
-        !grads->vf_b2 || !grads->vf_w3 || !grads->vf_b3 || (!p->discrete && !grads->logstd)) { srl_set_error("ppo2_grad: null gradient pointer"); return 1; }
-    const int ctas = grid_ctas(minibatch);
-    if (ctas <= 0) { srl_set_error("ppo2_grad: no CUDA device"); return 1; }
+    const int ctas = grad_args_ok("ppo2_grad", p, grads, minibatch);
+    if (ctas <= 0) return 1;
     const Seg seg = make_seg(p->obs_dim, p->n_out, p->discrete);
     if (workspace_bytes < 2048 + sizeof(float) * (size_t)seg.P * (size_t)ctas) { srl_set_error("ppo2_grad: workspace too small (srl_ppo2_workspace_bytes)"); return 1; }
     cudaStream_t st = (cudaStream_t)stream;
@@ -600,19 +684,50 @@ int srl_ppo2_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int minib
     GradArgs a;
     a.p = *p; a.mb = minibatch; a.idx = reinterpret_cast<const long long*>(idx); a.obs = obs; a.act = actions; a.adv = adv; a.ret = ret;
     a.old_logp = old_logp; a.old_val = old_value; a.clip = cliprange; a.ent_coef = ent_coef; a.vf_coef = vf_coef; a.stats = stats; a.partial = partial;
-    if (p->obs_dim <= MAXD) {
-        constexpr size_t smem = grad_smem_bytes<MAXD>();
-        SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_kernel>(smem));
-        ppo2_grad_kernel<<<ctas, NT, smem, st>>>(a);
-    } else {
-        constexpr size_t smem = grad_smem_bytes<WIDE_D>();
-        SRL_CUDA_OK(srl_smem_opt_in<ppo2_grad_wide_kernel>(smem));
-        ppo2_grad_wide_kernel<<<ctas, NT, smem, st>>>(a);
+    return launch_grad<ppo2_grad_kernel, ppo2_grad_wide_kernel>(a, grads, ctas, st);
+}
+
+size_t srl_a2c_workspace_bytes(int obs_dim, int n_out, int discrete, int rows) {
+    if (obs_dim < 1 || obs_dim > WIDE_D || n_out < 1 || n_out > MAXO || rows < 1) {
+        srl_set_error("a2c_workspace_bytes: unsupported shape obs_dim=%d n_out=%d rows=%d (obs_dim 1..%d, n_out 1..%d)", obs_dim, n_out, rows, WIDE_D, MAXO);
+        return 0;
     }
-    SRL_CUDA_OK(cudaGetLastError());
-    ReduceArgs r;
-    r.g = *grads; r.seg = seg; r.nparts = ctas; r.partial = partial;
-    ppo2_reduce_kernel<<<(seg.P + 255) / 256, 256, 0, st>>>(r);
+    const int ctas = grid_ctas(rows);
+    return sizeof(float) * (size_t)make_seg(obs_dim, n_out, discrete).P * (size_t)(ctas > 0 ? ctas : 1);
+}
+
+int srl_a2c_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int rows, const int64_t* idx, const float* obs, const void* actions,
+                 const float* ret, const float* old_value, float ent_coef, float vf_coef, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!p || !grads || !obs || !actions || !ret || !old_value || !workspace) { srl_set_error("a2c_grad: null argument"); return 1; }
+    const int ctas = grad_args_ok("a2c_grad", p, grads, rows);
+    if (ctas <= 0) return 1;
+    const Seg seg = make_seg(p->obs_dim, p->n_out, p->discrete);
+    if (workspace_bytes < sizeof(float) * (size_t)seg.P * (size_t)ctas) { srl_set_error("a2c_grad: workspace too small (srl_a2c_workspace_bytes)"); return 1; }
+    GradArgs a = {};
+    a.p = *p; a.mb = rows; a.idx = reinterpret_cast<const long long*>(idx); a.obs = obs; a.act = actions; a.ret = ret; a.old_val = old_value;
+    a.ent_coef = ent_coef; a.vf_coef = vf_coef; a.partial = reinterpret_cast<float*>(workspace);
+    return launch_grad<a2c_grad_kernel, a2c_grad_wide_kernel>(a, grads, ctas, (cudaStream_t)stream);
+}
+
+int srl_clip_rmsprop(int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, const srl_mlp_grads* grads, const srl_mlp_grads* ms,
+                     const float* lr, float max_grad_norm, float alpha, float epsilon, void* stream) {
+    if (!params || !grads || !ms || !lr) { srl_set_error("clip_rmsprop: null argument"); return 1; }
+    if (params->struct_size != sizeof(srl_mlp_grads) || grads->struct_size != sizeof(srl_mlp_grads) || ms->struct_size != sizeof(srl_mlp_grads)) {
+        srl_set_error("clip_rmsprop: struct size mismatch"); return 1;
+    }
+    if (obs_dim < 1 || obs_dim > WIDE_D || n_out < 1 || n_out > MAXO || (discrete && n_out < 2)) {
+        srl_set_error("clip_rmsprop: unsupported shape obs_dim=%d n_out=%d (obs_dim 1..%d, n_out 1..%d)", obs_dim, n_out, WIDE_D, MAXO); return 1;
+    }
+    if (!(max_grad_norm > 0.f) || !(alpha >= 0.f && alpha <= 1.f) || !(epsilon >= 0.f)) {
+        srl_set_error("clip_rmsprop: need max_grad_norm > 0, 0 <= alpha <= 1, epsilon >= 0 (got %g, %g, %g)", max_grad_norm, alpha, epsilon); return 1;
+    }
+    for (const srl_mlp_grads* t : {params, grads, ms}) {
+        if (!t->pi_w1 || !t->pi_b1 || !t->pi_w2 || !t->pi_b2 || !t->pi_w3 || !t->pi_b3 || !t->vf_w1 || !t->vf_b1 || !t->vf_w2 || !t->vf_b2 || !t->vf_w3 ||
+            !t->vf_b3 || (!discrete && !t->logstd)) { srl_set_error("clip_rmsprop: null tensor pointer"); return 1; }
+    }
+    OptArgs o;
+    o.p = *params; o.g = *grads; o.ms = *ms; o.seg = make_seg(obs_dim, n_out, discrete); o.lr = lr; o.max_norm = max_grad_norm; o.alpha = alpha; o.eps = epsilon;
+    clip_rmsprop_kernel<<<1, OPT_NT, 0, (cudaStream_t)stream>>>(o);
     SRL_CUDA_OK(cudaGetLastError());
     return 0;
 }

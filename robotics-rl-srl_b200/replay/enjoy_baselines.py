@@ -1,7 +1,8 @@
 """
 Mirror of the reference's replay entry point ``python -m replay.enjoy_baselines --log-dir <trained agent>``
 (replay/enjoy_baselines.py:45-63 arguments, :66-118 config loading, :151-333 the enjoy loop) for the agents this repo can
-train: it reloads ``args.json`` / ``env_globals.json`` / ``ppo2_model.pt`` written by ``rl_baselines.ppo2.train``, rebuilds the
+train: it reloads ``args.json`` / ``env_globals.json`` / ``<algo>_model.pt`` written by ``rl_baselines.ppo2.train`` or ``rl_baselines.a2c.train``
+(the same MlpPolicy), rebuilds the
 env batch with the training-time keyword arguments and the saved observation filter (``load_path_normalise``, :145), runs the
 policy for ``--num-timesteps`` steps and reports ``"<n> episodes - Mean reward: <r>"`` like the reference (:330-333).
 Rendering / plotting flags are accepted and ignored (image observations are out of scope, DESIGN.md section 8).
@@ -39,12 +40,13 @@ def loadConfigAndSetup(load_args):
         env_globals = json.load(f)
     with open(os.path.join(log_dir, "args.json")) as f:
         train_args = json.load(f)
-    if train_args.get("algo", "ppo2") != "ppo2":
-        raise ValueError(train_args.get("algo") + " is not supported for replay")
+    algo = train_args.get("algo", "ppo2")
+    if algo not in ("ppo2", "a2c"):
+        raise ValueError(algo + " is not supported for replay")
     env_kwargs = dict(env_globals)
     env_kwargs["shape_reward"] = load_args.shape_reward            # reward sparse or shaped: chosen at replay time (:88)
     env_kwargs["srl_model"] = train_args.get("srl_model", "ground_truth")
-    return train_args, os.path.join(log_dir, "ppo2_model.pt"), env_kwargs
+    return train_args, os.path.join(log_dir, algo + "_model.pt"), env_kwargs
 
 
 def main(argv=None):

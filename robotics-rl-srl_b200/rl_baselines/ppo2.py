@@ -130,6 +130,220 @@ def allreduce_mean_gradients(params, dist, world):
         off += n
 
 
+# ---- pieces shared with rl_baselines/a2c.py: the run's envs, policy and first observation, the collection loop, and the per-update
+#      bookkeeping (monitor log, episode statistics, best-model callback, saved model and run files) ----
+
+def make_run(algo, env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, fused_flags):
+    """The envs of this process (global env offset ``rank * num_envs``) and a policy over rows of ``num_stack * D`` values, identical on
+    every rank.  ``fused_flags``: the trainer's fused-path switches (None: on whenever the envs live on a GPU); rows wider than the fused
+    kernels take are refused when any is on.  Call after ``torch.manual_seed(seed)``; reseeds with ``seed + rank`` when data-parallel."""
+    env_kwargs = dict(env_kwargs or {})
+    dist, rank, world = _dist_world()
+    if prefetch_resets is None:
+        from srl_sim.backend import default_backend
+        prefetch_resets = default_backend(device).on_gpu
+    if prefetch_resets:
+        env_kwargs["prefetch_resets"] = True
+    if env_kwargs.get("srl_model", "ground_truth") != "ground_truth":
+        # the collection loop feeds the simulator's observation buffer (the 3-D / 2-D ground-truth observation) straight to the policy
+        raise ValueError("%s.train supports srl_model='ground_truth' only (got %r)" % (algo, env_kwargs["srl_model"]))
+    import types
+    from rl_baselines.utils import createTensorEnvs
+    env = createTensorEnvs(types.SimpleNamespace(env=env_id, num_cpu=num_envs, seed=seed, device=device), env_kwargs=env_kwargs,
+                           global_env_offset=rank * num_envs)
+    on_gpu = env.backend.on_gpu
+    # device -1 is the CPU oracle installed by a test through srl_sim.backend.use_library (its buffers are numpy arrays,
+    # shared with torch below); the product backend is always a CUDA device
+    dev = env.backend.torch_device if on_gpu else torch.device("cpu")
+    e_obs, e_rew, e_done, e_ep_ret, e_ep_len = [x if on_gpu else torch.from_numpy(x) for x in (env._obs, env._rew, env._done, env._ep_ret, env._ep_len)]
+    D = env.observation_space.shape[0]
+    K = int(num_stack)
+    if K < 1:
+        raise ValueError("num_stack must be >= 1 (got %d)" % K)
+    W = K * D                                  # the width of what the policy sees: the stacked row
+    if W > 32 and any(on_gpu if f is None else f for f in fused_flags):
+        from srl_sim.policy import MAX_OBS
+        raise ValueError("num_stack=%d x %d-wide observations = %d: the fused policy kernels take at most %d values per row" % (K, D, W, MAX_OBS))
+    if env.is_discrete:
+        policy = MlpPolicy(W, n_actions=env.action_space.n).to(dev)
+    else:
+        policy = MlpPolicy(W, action_dim=env.action_space.shape[0]).to(dev)
+    if dist is not None:
+        for p in policy.parameters():         # same seed => same init; the broadcast makes it independent of library versions
+            dist.broadcast(p.data, 0)
+        torch.manual_seed(seed + rank)        # action sampling / minibatch permutations differ per rank
+    return types.SimpleNamespace(algo=algo, env_id=env_id, num_envs=num_envs, env=env, env_kwargs=env_kwargs, prefetch_resets=prefetch_resets,
+                                 on_gpu=on_gpu, dev=dev, e_obs=e_obs, e_rew=e_rew, e_done=e_done, e_ep_ret=e_ep_ret, e_ep_len=e_ep_len,
+                                 D=D, K=K, W=W, policy=policy, dist=dist, rank=rank, world=world)
+
+
+def write_run_files(run, log_dir, num_timesteps, seed, hp):
+    """args.json and env_globals.json of the run directory (rank 0; rl_baselines/train.py:282-315 of the reference)."""
+    if log_dir and run.rank == 0:
+        os.makedirs(log_dir, exist_ok=True)
+        with open(os.path.join(log_dir, "args.json"), "w") as f:       # train.py:282-283
+            json.dump(dict(env=run.env_id, algo=run.algo, num_cpu=run.num_envs, num_timesteps=num_timesteps, seed=seed, srl_model="ground_truth",
+                           num_stack=run.K, **hp), f)
+        with open(os.path.join(log_dir, "env_globals.json"), "w") as f:  # train.py:285-315
+            json.dump({k: v for k, v in run.env_kwargs.items() if isinstance(v, (int, float, str, bool))}, f)
+
+
+def first_observation(run, norm):
+    """Reset every env; returns (the filtered observation, updated in place by the collection loop; the frame stack or None)."""
+    env, N, D, W = run.env, run.num_envs, run.D, run.W
+    env.sim.reset(obs_out=env._obs, stream=env.backend.stream())
+    row, stack = run.e_obs, None          # what the filter sees: the observation, or the frame stack over it
+    if run.K > 1:                         # VecFrameStack.reset: zeros, the first observation in the last D columns
+        stack = torch.zeros((N, W), device=run.dev)
+        stack[:, W - D:].copy_(run.e_obs)
+        row = stack
+    if run.dist is not None:              # the reset batch goes through the same merge, so every rank starts from one filter
+        prior = (norm.mean.clone(), norm.var.clone(), norm.count.clone())
+        norm.update(row)
+        merge_running_moments(norm, prior, run.dist.all_reduce, run.world)
+        obs = norm(row.clone(), update=False)
+    else:
+        obs = norm(row.clone())
+    return obs, stack
+
+
+def collect_rollout(run, norm, obs, stack, buf, last_val, fused=None, act_dev=None, done_u8=None):
+    """T lockstep env steps under the current policy into the [T, N, ...] rollout buffers ``buf``; everything stays on the device, nothing
+    synchronises.  With ``fused`` (srl_sim.policy.FusedPolicy) an env step is three launches -- policy step, simulator step, observation
+    filter (the frame stack in the same launch) -- and the simulator writes reward / done / episode return straight into the buffers;
+    otherwise the policy and the filter run in torch."""
+    env, policy, D, W = run.env, run.policy, run.D, run.W
+    T, N = buf["rew"].shape
+    with torch.no_grad():
+        if fused is not None:
+            st = env.backend.stream()          # torch's current stream: the capture's while a graph is captured
+            for t in range(T):
+                fused.act(N, obs, act_dev, buf["logp"][t], buf["val"][t], obs_buf=buf["obs"][t], act_buf=buf["act"][t], stream=st)
+                env.sim.step(act_dev, None, env._obs, buf["rew"][t], done_u8[t], buf["ep_ret"][t], buf["ep_len"][t], stream=st)
+                if run.K > 1:
+                    fused.stack_filter(N, env._obs, done_u8[t], stack, obs, update=True, stream=st)
+                else:
+                    fused.filter(N, env._obs, obs, update=True, stream=st)
+            buf["done"].copy_(done_u8)
+        else:
+            for t in range(T):
+                a, logp, v = policy.act(obs)
+                buf["obs"][t], buf["act"][t], buf["logp"][t], buf["val"][t] = obs, a, logp, v
+                a_env = a.to(torch.int32) if env.is_discrete else torch.clamp(a, -1, 1).contiguous()
+                env.step_tensors(a_env)                                   # one kernel launch, tensors stay on the GPU
+                buf["rew"][t], buf["done"][t], buf["ep_ret"][t], buf["ep_len"][t] = run.e_rew, run.e_done.float(), run.e_ep_ret, run.e_ep_len
+                if run.K > 1:                                             # VecFrameStack.step: roll by one frame, zero where done, newest frame last
+                    stack.copy_(torch.where(run.e_done.bool()[:, None], 0.0, torch.roll(stack, -D, 1)))
+                    stack[:, W - D:].copy_(run.e_obs)
+                    obs.copy_(norm(stack))
+                else:
+                    obs.copy_(norm(run.e_obs))
+        last_val.copy_(policy.vf(obs).squeeze(-1))
+
+
+def phase_timer(phase_times, on_gpu):
+    """tick(name, since): with a ``phase_times`` dict, synchronise and add the wall time since ``since`` to ``phase_times[name]``."""
+    def tick(name=None, since=0.0):
+        if phase_times is None:
+            return 0.0
+        if on_gpu:
+            torch.cuda.synchronize()
+        now = time.perf_counter()
+        if name is not None:
+            phase_times[name] = phase_times.get(name, 0.0) + now - since
+        return now
+    return tick
+
+
+class RunLog(object):
+    """The bookkeeping of a training run after each update: the monitor log (environments/utils.py:53-54 wraps every env in bench.Monitor;
+    rl_baselines/visualize.py:59-107 reads the files back: one ``<rank>.monitor.csv`` per process with the episodes of all its envs, return
+    and length straight from the kernel's episode statistics), the history of (steps, mean return of the last episodes, fps), the reference's
+    best-model callback (rl_baselines/train.py:132-159: every ``save_interval`` updates the mean return of the last N_EPISODES_EVAL episodes
+    of the monitor logs is computed, and when it beats the best so far and MIN_EPISODES_BEFORE_SAVE episodes exist the observation filter
+    and the model are saved as ``<algo>_model.pt``) and the files of the finished run."""
+    N_EPISODES_EVAL, MIN_EPISODES_BEFORE_SAVE = 100, 100
+
+    def __init__(self, run, norm, log_dir, save_interval, episode_window, verbose):
+        self.run, self.norm, self.log_dir, self.save_interval, self.episode_window, self.verbose = run, norm, log_dir, save_interval, episode_window, verbose
+        self.history, self.ep_returns = [], []
+        self.best_mean_reward, self.n_saved = -10000.0, 0
+        self.monitor = None
+        if log_dir:
+            from srl_sim.monitor import MonitorWriter
+            os.makedirs(log_dir, exist_ok=True)
+            self.monitor = MonitorWriter(os.path.join(log_dir, str(run.rank)), env_id=run.env_id)
+        self.t_start = time.time()
+
+    def start(self):
+        self.t_start = time.time()
+
+    def episodes(self, done, ep_ret, ep_len):
+        """The episodes that ended in the [steps, N] rows since the last call; their monitor times are spread over the wall time since then."""
+        dmask = done.bool()
+        new_rets = ep_ret[dmask].tolist()
+        self.ep_returns.extend(new_rets)
+        if self.monitor is not None and new_rets:
+            t_now = time.time() - self.monitor.t_start
+            t_idx = dmask.nonzero()[:, 0].float()                          # step index of each finished episode within the rows
+            t_prev = getattr(self.monitor, "_t_prev", 0.0)
+            self.monitor.write_episodes(new_rets, ep_len[dmask].tolist(), (t_prev + (t_now - t_prev) * (t_idx + 1.0) / done.shape[0]).tolist())
+            self.monitor._t_prev = t_now
+
+    def end_update(self, update, n_updates, steps, callback=True, print_every=1):
+        """History entry of update ``update`` (1-based) at ``steps`` global env steps, then -- with ``callback`` -- the best-model check when
+        the update is a multiple of ``save_interval``, then the progress line every ``print_every`` updates."""
+        run = self.run
+        fps = steps / (time.time() - self.t_start)
+        window = self.ep_returns[-max(self.episode_window, run.num_envs):]   # --episode_window (train.py:182), at least one episode per env
+        if run.dist is not None:
+            from srl_sim.distributed import allgather_episode_stats
+            mean_ret, n_ep = allgather_episode_stats(float(np.sum(window)), len(window), device=run.dev if run.on_gpu else None)
+            mean_ret = mean_ret if n_ep else float("nan")
+        else:
+            mean_ret = float(np.mean(window)) if window else float("nan")
+        self.history.append((steps, mean_ret, fps))
+        if callback and self.log_dir and update % self.save_interval == 0:
+            if run.dist is not None:
+                run.dist.barrier()             # every rank's monitor file holds this update's episodes
+            if run.rank == 0:
+                if run.dist is None:           # one process: the in-memory list is the monitor file (same episodes, same order)
+                    ok, n_episodes = len(self.ep_returns) > 0, len(self.ep_returns)
+                    eval_reward = float(np.mean(self.ep_returns[-self.N_EPISODES_EVAL:])) if ok else 0.0
+                else:
+                    from srl_sim.monitor import compute_mean_reward
+                    ok, eval_reward, n_episodes = compute_mean_reward(self.log_dir, self.N_EPISODES_EVAL)
+                if ok and self.verbose:
+                    print("Best mean reward: {:.2f} - Last mean reward per episode: {:.2f}".format(self.best_mean_reward, eval_reward))
+                if ok and eval_reward > self.best_mean_reward and n_episodes >= self.MIN_EPISODES_BEFORE_SAVE:
+                    self.best_mean_reward = eval_reward
+                    if self.verbose:
+                        print("Saving new best model")
+                    self.save_model(os.path.join(self.log_dir, "%s_model.pt" % run.algo))
+                    self.n_saved += 1
+        if self.verbose and run.rank == 0 and (update == n_updates or update % print_every == 0):
+            print("update %d/%d  steps %d  mean episode return %.3f  episodes %d  fps %.0f" % (update, n_updates, steps, mean_ret, len(self.ep_returns), fps))
+
+    def save_model(self, path):
+        from rl_baselines.utils import save_obs_rms
+        norm = self.norm
+        torch.save(dict(policy=self.run.policy.state_dict(), obs_mean=norm.mean.clone(), obs_var=norm.var.clone(), obs_count=norm.count.clone()), path)
+        save_obs_rms(self.log_dir, norm.mean.detach().cpu().numpy(), norm.var.detach().cpu().numpy(), float(norm.count))
+
+    def finish(self):
+        """Close the monitor; rank 0 saves ``<algo>_model_final.pt`` (and ``<algo>_model.pt`` if the callback never saved) and best_model.json."""
+        if self.monitor is not None:
+            self.monitor.close()
+        if self.log_dir and self.run.rank == 0:
+            algo = self.run.algo
+            self.save_model(os.path.join(self.log_dir, "%s_model_final.pt" % algo))
+            if self.n_saved == 0:              # a run too short for the callback to fire (fewer than MIN_EPISODES_BEFORE_SAVE episodes): keep the last model
+                self.save_model(os.path.join(self.log_dir, "%s_model.pt" % algo))
+            with open(os.path.join(self.log_dir, "best_model.json"), "w") as f:
+                json.dump(dict(best_mean_reward=self.best_mean_reward if self.n_saved else None, saves=self.n_saved, n_episodes_eval=self.N_EPISODES_EVAL,
+                               min_episodes_before_save=self.MIN_EPISODES_BEFORE_SAVE, save_interval_updates=self.save_interval), f)
+
+
 def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None, device=0, hyperparams=None, verbose=1, cuda_graph=True,
           phase_times=None, fused_act=None, prefetch_resets=None, episode_window=40, fused_update=None, num_stack=1):
     """PPO2.learn on a BatchedSRLVecEnv.  Returns a history of (timesteps, mean episode return, fps).
@@ -156,42 +370,10 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     ``collect`` / ``gae`` / ``optimise`` in it (a profiling aid: the synchronisations cost throughput)."""
     hp = dict(PPO2_DEFAULTS); hp.update(hyperparams or {})
     torch.manual_seed(seed)
-    env_kwargs = dict(env_kwargs or {})
-    dist, rank, world = _dist_world()
-    if prefetch_resets is None:
-        from srl_sim.backend import default_backend
-        prefetch_resets = default_backend(device).on_gpu
-    if prefetch_resets:
-        env_kwargs["prefetch_resets"] = True
-    if env_kwargs.get("srl_model", "ground_truth") != "ground_truth":
-        # the collection loop feeds the simulator's observation buffer (the 3-D / 2-D ground-truth observation) straight to the policy
-        raise ValueError("ppo2.train supports srl_model='ground_truth' only (got %r)" % env_kwargs["srl_model"])
-    import types
-    from rl_baselines.utils import createTensorEnvs, save_obs_rms
-    env = createTensorEnvs(types.SimpleNamespace(env=env_id, num_cpu=num_envs, seed=seed, device=device), env_kwargs=env_kwargs,
-                           global_env_offset=rank * num_envs)
-    on_gpu = env.backend.on_gpu
-    # device -1 is the CPU oracle installed by a test through srl_sim.backend.use_library (its buffers are numpy arrays,
-    # shared with torch below); the product backend is always a CUDA device
-    dev = env.backend.torch_device if on_gpu else torch.device("cpu")
-    e_obs, e_rew, e_done, e_ep_ret, e_ep_len = [x if on_gpu else torch.from_numpy(x) for x in (env._obs, env._rew, env._done, env._ep_ret, env._ep_len)]
-    D = env.observation_space.shape[0]
-    K = int(num_stack)
-    if K < 1:
-        raise ValueError("num_stack must be >= 1 (got %d)" % K)
-    W = K * D                                  # the width of what the policy sees: the stacked row
-    if W > 32 and ((on_gpu if fused_act is None else fused_act) or (on_gpu if fused_update is None else fused_update)):
-        from srl_sim.policy import MAX_OBS
-        raise ValueError("num_stack=%d x %d-wide observations = %d: the fused policy kernels take at most %d values per row" % (K, D, W, MAX_OBS))
-    if env.is_discrete:
-        policy = MlpPolicy(W, n_actions=env.action_space.n).to(dev)
-    else:
-        policy = MlpPolicy(W, action_dim=env.action_space.shape[0]).to(dev)
+    run = make_run("ppo2", env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, [fused_act, fused_update])
+    env, on_gpu, dev, policy, dist, rank, world = run.env, run.on_gpu, run.dev, run.policy, run.dist, run.rank, run.world
+    prefetch_resets, K, W = run.prefetch_resets, run.K, run.W
     params = list(policy.parameters())
-    if dist is not None:
-        for p in params:                      # same seed => same init; the broadcast makes it independent of library versions
-            dist.broadcast(p.data, 0)
-        torch.manual_seed(seed + rank)        # action sampling / minibatch permutations differ per rank
     N, T = num_envs, hp["n_steps"]
     # The GAE recursion and the minibatch step (forward, losses, backward, gradient clip, Adam) are captured into CUDA graphs too:
     # ~1000 and ~150 small launches respectively that cost more on the host than on the GPU.  Data-parallel runs keep the eager
@@ -204,25 +386,8 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         opt = torch.optim.Adam(params, lr=hp["learning_rate"], eps=1e-5)
     norm = RunningNorm(W, dev)
     n_updates = max(1, int(num_timesteps) // (N * T * world))
-    if log_dir and rank == 0:
-        os.makedirs(log_dir, exist_ok=True)
-        with open(os.path.join(log_dir, "args.json"), "w") as f:       # train.py:282-283
-            json.dump(dict(env=env_id, algo="ppo2", num_cpu=N, num_timesteps=num_timesteps, seed=seed, srl_model="ground_truth", num_stack=K, **hp), f)
-        with open(os.path.join(log_dir, "env_globals.json"), "w") as f:  # train.py:285-315
-            json.dump({k: v for k, v in env_kwargs.items() if isinstance(v, (int, float, str, bool))}, f)
-    env.sim.reset(obs_out=env._obs, stream=env.backend.stream())
-    row = e_obs                           # what the filter sees: the observation, or the frame stack over it
-    if K > 1:                             # VecFrameStack.reset: zeros, the first observation in the last D columns
-        stack = torch.zeros((N, W), device=dev)
-        stack[:, W - D:].copy_(e_obs)
-        row = stack
-    if dist is not None:                   # the reset batch goes through the same merge, so every rank starts from one filter
-        prior = (norm.mean.clone(), norm.var.clone(), norm.count.clone())
-        norm.update(row)
-        merge_running_moments(norm, prior, dist.all_reduce, world)
-        obs = norm(row.clone(), update=False)
-    else:
-        obs = norm(row.clone())          # the current (filtered) observation; updated IN PLACE by the collection loop
+    write_run_files(run, log_dir, num_timesteps, seed, hp)
+    obs, stack = first_observation(run, norm)    # the current (filtered) observation; updated IN PLACE by the collection loop
     buf = dict(obs=torch.empty((T, N, W), device=dev), act=torch.empty((T, N) if env.is_discrete else (T, N, env.sim.action_dim), device=dev,
                                                                        dtype=torch.int64 if env.is_discrete else torch.float32),
                logp=torch.empty((T, N), device=dev), val=torch.empty((T, N), device=dev), rew=torch.empty((T, N), device=dev),
@@ -243,39 +408,12 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         env.sim.prefetch_resets(stream=env.backend.stream())   # bulk fill of the first records; from here on the helper slots of every step launch keep them up
 
     def collect():
-        """n_steps lockstep env steps under the current policy; everything stays on the device, nothing synchronises."""
-        with torch.no_grad():
-            for t in range(T):
-                a, logp, v = policy.act(obs)
-                buf["obs"][t], buf["act"][t], buf["logp"][t], buf["val"][t] = obs, a, logp, v
-                act_dev = a.to(torch.int32) if env.is_discrete else torch.clamp(a, -1, 1).contiguous()
-                env.step_tensors(act_dev)                                 # one kernel launch, tensors stay on the GPU
-                buf["rew"][t], buf["done"][t], buf["ep_ret"][t], buf["ep_len"][t] = e_rew, e_done.float(), e_ep_ret, e_ep_len
-                if K > 1:                                                 # VecFrameStack.step: roll by one frame, zero where done, newest frame last
-                    stack.copy_(torch.where(e_done.bool()[:, None], 0.0, torch.roll(stack, -D, 1)))
-                    stack[:, W - D:].copy_(e_obs)
-                    obs.copy_(norm(stack))
-                else:
-                    obs.copy_(norm(e_obs))
-            last_val.copy_(policy.vf(obs).squeeze(-1))
+        """n_steps lockstep env steps under the current policy (three launches per env step on the fused path)."""
+        if fused is not None:
+            collect_rollout(run, norm, obs, stack, buf, last_val, fused=fused, act_dev=act_dev, done_u8=done_u8)
+        else:
+            collect_rollout(run, norm, obs, stack, buf, last_val)
 
-    def collect_fused():
-        """The same rollout as ``collect`` in three launches per env step: policy step, simulator step, observation filter.  The
-        simulator writes reward / done / episode return straight into the rollout buffers."""
-        with torch.no_grad():
-            st = env.backend.stream()
-            for t in range(T):
-                fused.act(N, obs, act_dev, buf["logp"][t], buf["val"][t], obs_buf=buf["obs"][t], act_buf=buf["act"][t], stream=st)
-                env.sim.step(act_dev, None, env._obs, buf["rew"][t], done_u8[t], buf["ep_ret"][t], buf["ep_len"][t], stream=st)
-                if K > 1:
-                    fused.stack_filter(N, env._obs, done_u8[t], stack, obs, update=True, stream=st)
-                else:
-                    fused.filter(N, env._obs, obs, update=True, stream=st)
-            buf["done"].copy_(done_u8)
-            last_val.copy_(policy.vf(obs).squeeze(-1))
-
-    if fused is not None:
-        collect = collect_fused
     graph = None
     if cuda_graph and on_gpu:
         # an even number of simulator launches per replay keeps the MobileRobot state double buffer (swapped by the host at every
@@ -286,7 +424,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(3):
-                policy.act(obs); norm(row, update=False)
+                policy.act(obs); norm(run.e_obs if stack is None else stack, update=False)
             if fused is not None:         # first launches outside the capture (one-off function attributes); they change nothing that matters:
                 fused.act(N, obs, act_dev, buf["logp"][0], buf["val"][0], stream=env.backend.stream())     # scratch rows, one sampling counter
                 if K > 1:                 # a copy of the stack and a scratch output: the stack itself must not advance
@@ -366,35 +504,10 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
             gae()
     mb_graph, mb_warm = None, 0        # the minibatch step is captured after three eager warm-up steps (real ones) on a side stream
 
-    history, ep_returns = [], []
-    # Monitor log (environments/utils.py:53-54 wraps every env in bench.Monitor; rl_baselines/visualize.py:59-107 reads the files back): one
-    # `<rank>.monitor.csv` per process with the episodes of all its envs, return and length straight from the kernel's episode statistics
-    monitor = None
-    if log_dir:
-        from srl_sim.monitor import MonitorWriter, compute_mean_reward
-        os.makedirs(log_dir, exist_ok=True)
-        monitor = MonitorWriter(os.path.join(log_dir, str(rank)), env_id=env_id)
-    # best-model callback of the reference (rl_baselines/train.py:132-159): every SAVE_INTERVAL callback calls (20 PPO2 updates of 8 envs x
-    # 128 steps there; scaled to this batch) the mean return of the last N_EPISODES_EVAL episodes of the monitor logs is computed, and when it
-    # beats the best so far (and MIN_EPISODES_BEFORE_SAVE episodes exist) the observation filter and the model are saved
-    N_EPISODES_EVAL, MIN_EPISODES_BEFORE_SAVE = 100, 100
-    save_interval = max(1, 20 * 8 * 128 // (N * T * world))
-    best_mean_reward, n_saved = -10000.0, 0
-
-    def save_model(path):
-        torch.save(dict(policy=policy.state_dict(), obs_mean=norm.mean.clone(), obs_var=norm.var.clone(), obs_count=norm.count.clone()), path)
-        save_obs_rms(log_dir, norm.mean.detach().cpu().numpy(), norm.var.detach().cpu().numpy(), float(norm.count))
-
-    def tick(name=None, since=0.0):
-        if phase_times is None:
-            return 0.0
-        if on_gpu:
-            torch.cuda.synchronize()
-        now = time.perf_counter()
-        if name is not None:
-            phase_times[name] = phase_times.get(name, 0.0) + now - since
-        return now
-    t_start = time.time()
+    # best-model callback every SAVE_INTERVAL callback calls of the reference: 20 PPO2 updates of 8 envs x 128 steps there, scaled to this batch
+    log = RunLog(run, norm, log_dir, max(1, 20 * 8 * 128 // (N * T * world)), episode_window, verbose)
+    tick = phase_timer(phase_times, on_gpu)
+    log.start()
     for update in range(1, n_updates + 1):
         frac = 1.0 - (update - 1.0) / n_updates
         if graph_update:
@@ -411,15 +524,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         if dist is not None:                   # one all-reduce of 2 D + 1 doubles per rollout
             merge_running_moments(norm, prior, dist.all_reduce, world)
         t_ph = tick("collect", t_ph)
-        dmask = buf["done"].bool()
-        new_rets = buf["ep_ret"][dmask].tolist()
-        ep_returns.extend(new_rets)
-        if monitor is not None and new_rets:
-            t_now = time.time() - monitor.t_start
-            t_idx = dmask.nonzero()[:, 0].float()                          # step index of each finished episode within the rollout
-            t_prev = getattr(monitor, "_t_prev", 0.0)
-            monitor.write_episodes(new_rets, buf["ep_len"][dmask].tolist(), (t_prev + (t_now - t_prev) * (t_idx + 1.0) / T).tolist())
-            monitor._t_prev = t_now
+        log.episodes(buf["done"], buf["ep_ret"], buf["ep_len"])
         if gae_graph is not None:
             gae_graph.replay()
         else:
@@ -451,45 +556,9 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
                         minibatch_step(idx_static)
                     mb_graph.replay()                  # the capture only recorded this minibatch: now run it
         t_ph = tick("optimise", t_ph)
-        steps = update * N * T * world
-        fps = steps / (time.time() - t_start)
-        window = ep_returns[-max(episode_window, N):]                      # --episode_window (train.py:182), at least one episode per env
-        if dist is not None:
-            from srl_sim.distributed import allgather_episode_stats
-            mean_ret, n_ep = allgather_episode_stats(float(np.sum(window)), len(window), device=dev if on_gpu else None)
-            mean_ret = mean_ret if n_ep else float("nan")
-        else:
-            mean_ret = float(np.mean(window)) if window else float("nan")
-        history.append((steps, mean_ret, fps))
-        if log_dir and update % save_interval == 0:
-            if dist is not None:
-                dist.barrier()             # every rank's monitor file holds this update's episodes
-            if rank == 0:
-                if dist is None:           # one process: the in-memory list is the monitor file (same episodes, same order)
-                    ok, n_episodes = len(ep_returns) > 0, len(ep_returns)
-                    eval_reward = float(np.mean(ep_returns[-N_EPISODES_EVAL:])) if ok else 0.0
-                else:
-                    ok, eval_reward, n_episodes = compute_mean_reward(log_dir, N_EPISODES_EVAL)
-                if ok and verbose:
-                    print("Best mean reward: {:.2f} - Last mean reward per episode: {:.2f}".format(best_mean_reward, eval_reward))
-                if ok and eval_reward > best_mean_reward and n_episodes >= MIN_EPISODES_BEFORE_SAVE:
-                    best_mean_reward = eval_reward
-                    if verbose:
-                        print("Saving new best model")
-                    save_model(os.path.join(log_dir, "ppo2_model.pt"))
-                    n_saved += 1
-        if verbose and rank == 0:
-            print("update %d/%d  steps %d  mean episode return %.3f  episodes %d  fps %.0f" % (update, n_updates, steps, mean_ret, len(ep_returns), fps))
-    if monitor is not None:
-        monitor.close()
-    if log_dir and rank == 0:
-        save_model(os.path.join(log_dir, "ppo2_model_final.pt"))
-        if n_saved == 0:                   # a run too short for the callback to fire (fewer than MIN_EPISODES_BEFORE_SAVE episodes): keep the last model
-            save_model(os.path.join(log_dir, "ppo2_model.pt"))
-        with open(os.path.join(log_dir, "best_model.json"), "w") as f:
-            json.dump(dict(best_mean_reward=best_mean_reward if n_saved else None, saves=n_saved, n_episodes_eval=N_EPISODES_EVAL,
-                           min_episodes_before_save=MIN_EPISODES_BEFORE_SAVE, save_interval_updates=save_interval), f)
+        log.end_update(update, n_updates, update * N * T * world)
+    log.finish()
     env.close()
-    train.best_mean_reward, train.n_saved = best_mean_reward, n_saved
+    train.best_mean_reward, train.n_saved = log.best_mean_reward, log.n_saved
     train.last_policy, train.last_norm = policy, norm      # for callers that want the trained objects (tests, enjoy)
-    return history
+    return log.history

@@ -1,8 +1,8 @@
 """
 Mirror of the reference's training entry point ``python -m rl_baselines.train`` (rl_baselines/train.py:172-333) for the
-algorithms this repo provides as consumers of the simulator: ``ppo2`` (rl_baselines/ppo2.py) and ``random_agent``
-(rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the batch (per GPU when launched
-with ``torchrun --nproc-per-node N -m rl_baselines.train``: data-parallel PPO2, see rl_baselines/ppo2.py).
+algorithms this repo provides as consumers of the simulator: ``ppo2`` (rl_baselines/ppo2.py), ``a2c`` (rl_baselines/a2c.py) and
+``random_agent`` (rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the batch (per GPU when launched
+with ``torchrun --nproc-per-node N -m rl_baselines.train``: data-parallel PPO2 or A2C, see rl_baselines/ppo2.py).
 """
 import argparse
 import os
@@ -13,28 +13,35 @@ from environments.registry import registered_env
 # rl_baselines/rl_algorithm/ppo2.py:25-36 (getOptParam): the hyper-parameters `--hyperparam name:value` may set, and their types
 PPO2_OPT_PARAM = {"lam": float, "gamma": float, "max_grad_norm": float, "vf_coef": float, "learning_rate": float, "ent_coef": float,
                   "cliprange": float, "noptepochs": int, "n_steps": int}
+# rl_baselines/rl_algorithm/a2c.py (A2CModel.getOptParam)
+A2C_OPT_PARAM = {"n_steps": int, "vf_coef": float, "ent_coef": float, "max_grad_norm": float, "learning_rate": float, "epsilon": float,
+                 "alpha": float, "gamma": float, "lr_schedule": str}
+LR_SCHEDULES = ['linear', 'constant', 'double_linear_con', 'middle_drop', 'double_middle_drop']
 
 
-def parserHyperParam(pairs):
+def parserHyperParam(pairs, opt_param=PPO2_OPT_PARAM):
     """``["name:value", ...]`` -> typed dict (train.py:321 + base_classes.py:62-80: unknown names are an AssertionError)."""
     parsed = {}
     for param in pairs:
         name, val = param.split(":")[0], param.split(":")[1]
-        if name not in PPO2_OPT_PARAM:
+        if name not in opt_param:
             raise AssertionError("Error: hyperparameter {} not in list of valid hyperparameters".format(name))
-        parsed[name] = PPO2_OPT_PARAM[name](val)
+        parsed[name] = opt_param[name](val)
+    if parsed.get("lr_schedule", LR_SCHEDULES[0]) not in LR_SCHEDULES:
+        raise AssertionError("Error: lr_schedule {} not in {}".format(parsed["lr_schedule"], LR_SCHEDULES))
     return parsed
 
 
 def main(argv=None):
     parser = argparse.ArgumentParser(description="Train script for RL algorithms")
-    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'random_agent'], type=str)
+    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'a2c', 'random_agent'], type=str)
     parser.add_argument('--env', type=str, help='environment ID', default='KukaButtonGymEnv-v0', choices=list(registered_env.keys()))
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--episode_window', type=int, default=40, help='Episode window for moving average plot (default: 40)')
     parser.add_argument('--num-stack', type=int, default=1, help='number of frames to stack (default: 1)')
     parser.add_argument('-joints', '--action-joints', action='store_true', default=False, help='set actions to the joints of the arm directly')
-    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 hyper-parameters as name:value pairs')
+    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 / A2C hyper-parameters as name:value pairs')
+    parser.add_argument('--lr-schedule', help='Learning rate schedule (a2c)', default='constant', choices=LR_SCHEDULES)
     parser.add_argument('--log-dir', default='/tmp/gym/', type=str)
     parser.add_argument('--num-timesteps', type=int, default=int(1e6))
     parser.add_argument('--srl-model', type=str, default='ground_truth', choices=['ground_truth'])
@@ -52,15 +59,20 @@ def main(argv=None):
     assert args.action_repeat >= 1, "Error: --action-repeat cannot be less than 1"
     if args.action_joints and not args.continuous_actions:
         raise ValueError("The joints action space is continuous only: use '-joints' together with '-c' (kuka_button_gym_env.py:149-161)")
-    hyperparams = parserHyperParam(args.hyperparam)
+    hyperparams = parserHyperParam(args.hyperparam, A2C_OPT_PARAM if args.algo == "a2c" else PPO2_OPT_PARAM)
+    if args.algo == "a2c":
+        hyperparams = dict(dict(lr_schedule=args.lr_schedule), **hyperparams)
     env_kwargs = dict(is_discrete=not args.continuous_actions, action_repeat=args.action_repeat, random_target=args.random_target,
                       shape_reward=args.shape_reward, srl_model=args.srl_model)
     if args.action_joints:
         env_kwargs["action_joints"] = True
     log_dir = os.path.join(args.log_dir, args.env, args.srl_model, args.algo, time.strftime("%y-%m-%d_%Hh%M_%S"))
     num_timesteps = int(1.1 * args.num_timesteps)      # the reference trains 10 % longer (train.py:319)
-    if args.algo == "ppo2":
-        from rl_baselines.ppo2 import train
+    if args.algo in ("ppo2", "a2c"):
+        if args.algo == "ppo2":
+            from rl_baselines.ppo2 import train
+        else:
+            from rl_baselines.a2c import train
         from srl_sim.distributed import rank_world
         rank, world, local_rank = rank_world()
         device = args.device

@@ -12,7 +12,9 @@ import ctypes
 from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64, c_void_p
 
 HIDDEN, MAX_OBS, MAX_OUT = 64, 32, 8     # observation widths 1..8 and 9..32 (stacked states) run separate kernel instantiations
-POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae"]
+POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae",
+                  "srl_a2c_grad", "srl_a2c_workspace_bytes", "srl_clip_rmsprop"]
+GRAD_NAMES = ["pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3", "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3", "logstd"]
 
 
 class SrlMlpPolicy(Structure):
@@ -44,7 +46,31 @@ def bind(cdll):
                                    c_float, c_float, c_float, c_void_p, c_size_t, c_void_p]
     cdll.srl_ppo2_gae.restype = c_int
     cdll.srl_ppo2_gae.argtypes = [c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_void_p, c_void_p, c_void_p]
+    cdll.srl_a2c_workspace_bytes.restype = c_size_t
+    cdll.srl_a2c_workspace_bytes.argtypes = [c_int, c_int, c_int, c_int]
+    cdll.srl_a2c_grad.restype = c_int
+    cdll.srl_a2c_grad.argtypes = [POINTER(SrlMlpPolicy), POINTER(SrlMlpGrads), c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float,
+                                  c_void_p, c_size_t, c_void_p]
+    cdll.srl_clip_rmsprop.restype = c_int
+    cdll.srl_clip_rmsprop.argtypes = [c_int, c_int, c_int, POINTER(SrlMlpGrads), POINTER(SrlMlpGrads), POINTER(SrlMlpGrads), c_void_p, c_float, c_float,
+                                      c_float, c_void_p]
     return cdll
+
+
+def policy_params(policy):
+    """The parameters of an MlpPolicy in the order of ``srl_mlp_grads`` (logstd last, Box only)."""
+    lin = lambda tower: [m for m in tower if hasattr(m, "weight")]
+    params = [t for layer in lin(policy.pi) + lin(policy.vf) for t in (layer.weight, layer.bias)]
+    return params if policy.discrete else params + [policy.logstd]
+
+
+def tensors_struct(tensors):
+    """``srl_mlp_grads`` over 12 or 13 tensors in the order of :func:`policy_params` (gradients, parameters or optimiser slots)."""
+    s = SrlMlpGrads()
+    s.struct_size = ctypes.sizeof(SrlMlpGrads)
+    for name, t in zip(GRAD_NAMES, tensors):
+        setattr(s, name, t.data_ptr())
+    return s
 
 
 def policy_struct(policy):
@@ -123,6 +149,7 @@ class FusedPPO2Grad(object):
     """``srl_ppo2_grad``: the gradient of the PPO2 loss over one minibatch in one pass (forward, loss derivative, backward of both towers
     with every activation on chip), written into the policy's ``.grad`` tensors -- what ``loss.backward()`` of
     ``rl_baselines.ppo2``'s minibatch step produces.  Gradient clipping and the optimiser step stay with torch."""
+    _workspace_fn = "srl_ppo2_workspace_bytes"
 
     def __init__(self, library, policy, minibatch):
         import torch
@@ -132,21 +159,15 @@ class FusedPPO2Grad(object):
         dev = policy.pi[0].weight.device
         if dev.type != "cuda":
             raise ValueError("FusedPPO2Grad needs a policy on a CUDA device (there is no CPU fallback)")
-        lin = lambda tower: [m for m in tower if hasattr(m, "weight")]
-        params = [t for layer in lin(policy.pi) + lin(policy.vf) for t in (layer.weight, layer.bias)]
-        if not policy.discrete:
-            params.append(policy.logstd)
-        self.grads = SrlMlpGrads()
-        self.grads.struct_size = ctypes.sizeof(SrlMlpGrads)
-        names = ["pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3", "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3"] + ([] if policy.discrete else ["logstd"])
-        for name, prm in zip(names, params):
+        params = policy_params(policy)
+        for prm in params:
             prm.grad = torch.zeros_like(prm)               # static gradient tensors: the kernel overwrites them, the optimiser reads them (capturable)
-            setattr(self.grads, name, prm.grad.data_ptr())
+        self.grads = tensors_struct([prm.grad for prm in params])
         self.params = params
         self.minibatch = int(minibatch)
-        nbytes = int(self._lib.srl_ppo2_workspace_bytes(self.struct.obs_dim, self.struct.n_out, self.struct.discrete, self.minibatch))
+        nbytes = int(getattr(self._lib, self._workspace_fn)(self.struct.obs_dim, self.struct.n_out, self.struct.discrete, self.minibatch))
         if nbytes <= 0:
-            raise ValueError("srl_ppo2_workspace_bytes: unsupported shape")
+            raise ValueError("%s: unsupported shape" % self._workspace_fn)
         self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
 
     def gae(self, rew, value, done, last_value, gamma, lam, adv_out, ret_out, stream=None):
@@ -162,3 +183,48 @@ class FusedPPO2Grad(object):
                                      actions.data_ptr(), adv.data_ptr(), ret.data_ptr(), old_logp.data_ptr(), old_value.data_ptr(),
                                      float(cliprange), float(ent_coef), float(vf_coef), self.workspace.data_ptr(), self.workspace.numel(), stream)
         self._library.check(rc, "srl_ppo2_grad")
+
+
+class FusedA2CGrad(FusedPPO2Grad):
+    """``srl_a2c_grad``: the gradient of stable-baselines' A2C loss over the rows of one update (advantage ``ret - old_value``, no
+    normalisation, no clipping; include/srl_policy.h), in the same kernels as :class:`FusedPPO2Grad` and into the same static ``.grad``
+    tensors.  ``minibatch`` is the number of rows of an update (n_steps x envs).  ``gae`` (lambda = 1) gives the returns."""
+    _workspace_fn = "srl_a2c_workspace_bytes"
+
+    def __call__(self, idx, obs, actions, ret, old_value, ent_coef, vf_coef, stream=None):
+        """CUDA tensors of the rollout (``idx``: int64 [rows], or None for the first ``minibatch`` rows)."""
+        rc = self._lib.srl_a2c_grad(byref(self.struct), byref(self.grads), self.minibatch, None if idx is None else idx.data_ptr(), obs.data_ptr(),
+                                    actions.data_ptr(), ret.data_ptr(), old_value.data_ptr(), float(ent_coef), float(vf_coef),
+                                    self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._library.check(rc, "srl_a2c_grad")
+
+
+class FusedClipRMSprop(object):
+    """``srl_clip_rmsprop``: TF1's ``clip_by_global_norm`` + ``RMSPropOptimizer`` (momentum 0) over every tensor of an MlpPolicy in one launch.
+    Reads the policy's ``.grad`` tensors (which must exist and stay put: :class:`FusedA2CGrad` makes them static), updates the parameters in
+    place and owns the RMSProp slots ``ms`` (initialised to 1.0 as TF does) and the learning rate ``lr`` (float32 [1] on the device, for
+    a captured step to follow a schedule)."""
+
+    def __init__(self, library, policy, max_grad_norm, alpha, epsilon, lr=None):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        self.params = policy_params(policy)
+        dev = self.params[0].device
+        if dev.type != "cuda":
+            raise ValueError("FusedClipRMSprop needs a policy on a CUDA device (there is no CPU fallback)")
+        if any(p.grad is None for p in self.params):
+            raise ValueError("FusedClipRMSprop needs the policy's .grad tensors (create them first, e.g. with FusedA2CGrad)")
+        st, _ = policy_struct(policy)
+        self.obs_dim, self.n_out, self.discrete = st.obs_dim, st.n_out, st.discrete
+        self.ms = [torch.ones_like(p) for p in self.params]
+        self.lr = torch.zeros(1, dtype=torch.float32, device=dev) if lr is None else lr
+        self._p, self._g, self._m = tensors_struct(self.params), tensors_struct([p.grad for p in self.params]), tensors_struct(self.ms)
+        self.max_grad_norm, self.alpha, self.epsilon = float(max_grad_norm), float(alpha), float(epsilon)
+
+    def __call__(self, lr=None, stream=None):
+        """One step with the learning rate in ``lr`` (a float32 device scalar; default: this object's ``lr``)."""
+        lr = self.lr if lr is None else lr
+        rc = self._lib.srl_clip_rmsprop(self.obs_dim, self.n_out, self.discrete, byref(self._p), byref(self._g), byref(self._m), lr.data_ptr(),
+                                        self.max_grad_norm, self.alpha, self.epsilon, stream)
+        self._library.check(rc, "srl_clip_rmsprop")
