@@ -15,6 +15,10 @@
  *   srl_a2c_grad    <- the loss + `tf.gradients` of stable-baselines 2.5 `A2C.setup_model`, run once per update by `A2C._train_step`
  *                      (chosen by rl_baselines/rl_algorithm/a2c.py)
  *   srl_clip_rmsprop <- the same `_train_step`'s `tf.clip_by_global_norm` + `tf.train.RMSPropOptimizer` apply op
+ *   srl_dqn_act, srl_replay_add, srl_replay_sample, srl_dqn_target, srl_dqn_grad, srl_replay_update, srl_clip_adam
+ *                   <- stable-baselines 2.5 `DQN.learn` with the deepq `MlpPolicy` (chosen by rl_baselines/rl_algorithm/deepq.py): the
+ *                      epsilon-greedy `act`, baselines' `PrioritizedReplayBuffer` (add, sample, update_priorities) and `build_train`'s double-Q
+ *                      loss, `tf.clip_by_norm` per gradient tensor and `tf.train.AdamOptimizer`
  *
  * Conventions are those of srl_sim.h: 0 on success, message from srl_sim_last_error(); all pointers are DEVICE pointers;
  * calls are asynchronous on `stream` and capturable into a CUDA graph (everything a launch reads that changes between
@@ -132,6 +136,79 @@ int srl_clip_rmsprop(int obs_dim, int n_out, int discrete, const srl_mlp_grads* 
  * (stable-baselines' `discount_with_dones` over the rewards followed by the last value). */
 int srl_ppo2_gae(int n_steps, int n_envs, const float* rew, const float* value, const float* done, const float* last_value, double gamma, double lam,
                  float* adv_out, float* ret_out, void* stream);
+
+/* ---- DQN (rl_baselines/deepq.py) ----
+ * The Q network is an srl_mlp_policy with discrete = 1, n_out = the number of actions (2..8), obs_dim 1..32: the pi tower is the advantage head
+ * A (n_out values), the vf tower the state value V, both obs_dim -> 64 -> 64 with ReLU (not tanh), and
+ *   Q = V + (A - mean(A)),   mean(A) = (A_0 + ... + A_{n-1}) * (1 / n) in float32, summed in order.
+ * RECALLED from stable-baselines 2.5 / baselines, not checked against an installed copy (none can be installed here): the dueling head and the
+ * ReLU towers of the deepq MlpPolicy (layers [64, 64], no layer norm), double Q in build_train, the Huber loss with delta 1, tf.clip_by_norm
+ * per tensor, TF1 Adam's update order, and baselines' PrioritizedReplayBuffer / SegmentTree.  Every entry point refuses discrete = 0. */
+
+/* The epsilon-greedy step for n envs: Q of obs (f32[n, obs_dim]); env i draws from the Philox stream (seed, env_offset + i, counter) with purpose 24:
+ * a 53-bit uniform from words 0-1 below *eps explores, and then the action is (word 2 * n_out) >> 32, otherwise argmax Q (ties: the lowest index).
+ *   eps     : f32[1] device scalar;  rng : u64[3] {seed, counter, 0}, the counter advances by one per launch as for srl_policy_act
+ *   obs_buf : nullable f32[n, obs_dim] copy of obs;  act_env : i32[n];  act_buf : nullable i64[n];  q_out : nullable f32[n, n_out], Q itself */
+int srl_dqn_act(const srl_mlp_policy* q, int n, const float* obs, const float* eps, uint64_t* rng, uint64_t env_offset, float* obs_buf,
+                int32_t* act_env, int64_t* act_buf, float* q_out, void* stream);
+
+/* The double-Q target of `batch` sampled transitions: for row g = idx[b] (idx NULL: g = b), b* = argmax Q_online(next_obs[g]) and
+ *   y[b] = rew[g] + gamma * ((1 - done[g]) * Q_target(next_obs[g], b*))   (float32, in this order of roundings).
+ *   next_obs : f32[rows, obs_dim];  rew : f32[rows];  done : u8[rows];  y : f32[batch] */
+int srl_dqn_target(const srl_mlp_policy* online, const srl_mlp_policy* target, int batch, const int64_t* idx, const float* next_obs, const float* rew,
+                   const uint8_t* done, float gamma, float* y, void* stream);
+
+/* The gradient of loss = mean(w * huber(td)), td = Q(obs[g], act[g]) - y[b], over `batch` samples, written into `grads` like srl_a2c_grad (the same
+ * kernels, chunking and deterministic CTA-order reduction; ReLU towers, and per sample the head derivatives g = w clamp(td, -1, 1) / batch,
+ * d/dA_k = g ([k = act] - 1 / n), d/dV = g).
+ *   idx : nullable i64[batch] rows;  obs : f32[rows, obs_dim];  actions : i64[rows];  y, weights : f32[batch] in batch order (weights NULL: 1)
+ *   td_out : f32[batch], td of every sample;  workspace : at least srl_a2c_workspace_bytes(obs_dim, n_out, 1, batch) bytes (no state between calls) */
+int srl_dqn_grad(const srl_mlp_policy* q, const srl_mlp_grads* grads, int batch, const int64_t* idx, const float* obs, const int64_t* actions,
+                 const float* y, const float* weights, float* td_out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* One optimiser step of stable-baselines' DQN over every tensor of the Q network (discrete = 1; discrete = 0 is refused), in one launch: per tensor g = t * clip_norm / max(l2norm(t), clip_norm)
+ * (tf.clip_by_norm; l2norm summed in float64, rounded to float32; an infinite entry makes that entry NaN and the tensor's others 0, a NaN entry
+ * makes the whole tensor NaN; other tensors are unaffected), then TF1 Adam with slots m, v from 0:
+ *   m += (g - m)(1 - beta1);  v += (g^2 - v)(1 - beta2);  lr_t = lr sqrt(1 - beta2^t) / (1 - beta1^t);  w -= m lr_t / (sqrt(v) + epsilon)
+ * (epsilon outside the square root; not torch.optim.Adam's bias correction).
+ *   lr : f32[1] device scalar;  beta_power : f32[2] {beta1^t, beta2^t}, TF's accumulators: the caller starts them at {beta1, beta2}, every call
+ *   multiplies them by {beta1, beta2} after its step.  Two calls on the same inputs give the same bytes. */
+int srl_clip_adam(int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, const srl_mlp_grads* grads, const srl_mlp_grads* m,
+                  const srl_mlp_grads* v, const float* lr, float* beta_power, float clip_norm, float beta1, float beta2, float epsilon, void* stream);
+
+/* Prioritized replay over a ring of capacity = rows * n_envs transitions, row r holding transitions r * n_envs .. r * n_envs + n_envs - 1.
+ * Two float64 segment trees (baselines' SegmentTree): node 1 is the root, node k has children 2k and 2k + 1, leaf i sits at tree_cap + i, and
+ * every internal node is sum(left, right) / min(left, right).  The caller allocates and initialises the device words: sum 0, min +inf,
+ * max_priority 1, size 0, stamp -1. */
+typedef struct srl_replay_tree {
+    uint32_t struct_size;   /* = sizeof(srl_replay_tree); checked                                      */
+    int32_t  n_envs;        /* transitions per ring row                                                */
+    int64_t  capacity;      /* transitions the ring holds (a multiple of n_envs)                      */
+    int64_t  tree_cap;      /* leaves per tree: the power of two >= capacity                          */
+    double*  sum;           /* f64[2 tree_cap] (entry 0 unused)                                        */
+    double*  min;           /* f64[2 tree_cap]                                                         */
+    double*  max_priority;  /* f64[1]                                                                  */
+    int64_t* size;          /* i64[1]: transitions stored                                              */
+    int32_t* stamp;         /* i32[capacity]: srl_replay_update's scratch, -1 between calls            */
+} srl_replay_tree;
+
+/* The leaves of ring row `row` become max_priority^alpha (float64) in both trees, their ancestors are rebuilt and size becomes
+ * max(size, (row + 1) n_envs). */
+int srl_replay_add(const srl_replay_tree* t, int64_t row, double alpha, void* stream);
+
+/* `batch` i.i.d. samples; sample b draws a 53-bit uniform u from the Philox stream (seed, b, counter) with purpose 25 (rng as for srl_dqn_act).
+ *   prioritized: mass = u * sum[root], then find_prefixsum_idx (left child > mass: go left, else mass -= left, go right); a walk that float64
+ *                rounding ends in an empty leaf (index >= size) is clamped to size - 1.  w = (p_i size)^-beta / (p_min size)^-beta with
+ *                p = leaf / sum[root], p_min = min[root] / sum[root], in float64, rounded to float32.  beta : f64[1] device scalar.
+ *   otherwise:   i = min(floor(u size), size - 1), w = 1.
+ *   idx_out : i64[batch];  w_out : f32[batch] */
+int srl_replay_sample(const srl_replay_tree* t, int batch, int prioritized, const double* beta, uint64_t* rng, int64_t* idx_out, float* w_out,
+                      void* stream);
+
+/* After a gradient step: priority p = |td[b]| + eps in float32, leaf idx[b] = p^alpha in float64 in both trees (a leaf sampled twice takes the
+ * priority of its LAST occurrence in the batch), max_priority = max(max_priority, p), then every internal node is rebuilt bottom-up.
+ * idx entries must be stored transitions (0 <= idx < size). */
+int srl_replay_update(const srl_replay_tree* t, int batch, const int64_t* idx, const float* td, double alpha, float eps, void* stream);
 
 #ifdef __cplusplus
 }

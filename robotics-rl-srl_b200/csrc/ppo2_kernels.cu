@@ -40,6 +40,7 @@ struct GradArgs {
     float clip, ent_coef, vf_coef;
     const double* stats;      // STATS_CTAS x {sum(x - shift), sum((x - shift)^2)}, then the shift: the minibatch's advantages
     float* partial;           // [gridDim.x][P]
+    float* td;                // DQN: per-sample TD error out, [mb] in batch order
 };
 
 // ---- advantage statistics of the minibatch: STATS_CTAS partial sums (float64, about the first element: no cancellation), combined in a fixed
@@ -106,9 +107,12 @@ __device__ __forceinline__ float dot64(const float* row, const float* col) {
     return (s0 + s1) + (s2 + s3);
 }
 
+// the loss a gradient kernel instantiation differentiates (srl_ppo2_grad, srl_a2c_grad, srl_dqn_grad)
+enum LossKind { PPO2_LOSS, A2C_LOSS, DQN_LOSS };
+
 struct SampleRegs { float x[MAXD], af[MAXO], adv, ret, olp, ov; int ai, valid; };
 
-template <bool LOAD_X, bool A2C>
+template <bool LOAD_X, int L>
 __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs& r) {
     const int D = a.p.obs_dim, A = a.p.n_out;
     r.valid = s < a.mb;
@@ -127,7 +131,10 @@ __device__ __forceinline__ void load_sample(const GradArgs& a, int s, SampleRegs
             for (int k = 0; k < MAXO; ++k) if (k < A) r.af[k] = reinterpret_cast<const float*>(a.act)[g * A + k];
         }
     }
-    if constexpr (A2C) { r.adv = 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = 0.f; r.ov = r.valid ? a.old_val[g] : 0.f; }   // advantage: ret - old_val
+    if constexpr (L == A2C_LOSS) { r.adv = 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = 0.f; r.ov = r.valid ? a.old_val[g] : 0.f; }   // advantage: ret - old_val
+    else if constexpr (L == DQN_LOSS) {    // ret: the target y, ov: the importance weight (NULL: 1); both in batch order, not row order
+        r.adv = 0.f; r.ret = r.valid ? a.ret[s] : 0.f; r.olp = 0.f; r.ov = r.valid ? (a.old_val ? a.old_val[s] : 1.f) : 0.f;
+    }
     else { r.adv = r.valid ? a.adv[g] : 0.f; r.ret = r.valid ? a.ret[g] : 0.f; r.olp = r.valid ? a.old_logp[g] : 0.f; r.ov = r.valid ? a.old_val[g] : 0.f; }
 }
 
@@ -147,10 +154,18 @@ __device__ __forceinline__ void load_row_part(const GradArgs& a, int s, int u, f
     for (int j = 0; j < XQ; ++j) x[j] = (valid && u + 4 * j < D) ? a.obs[g * D + u + 4 * j] : 0.f;
 }
 
+// hidden activation of the towers and its derivative from the activation h: tanh (1 - h^2), or ReLU (TF's gradient: 0 where the
+// pre-activation is <= 0, i.e. where h = 0)
+template <int L>
+__device__ __forceinline__ float act_fn(float x) { if constexpr (L == DQN_LOSS) return fmaxf(x, 0.f); else return tanhf(x); }
+template <int L>
+__device__ __forceinline__ float dact_fn(float d, float h) { if constexpr (L == DQN_LOSS) return h > 0.f ? d : 0.f; else return d * (1.0f - h * h); }
+
 template <int MD>
 __host__ __device__ constexpr int grad_w1_stride() { return MD == MAXD ? MAXD : MD + 1; }
-// A2C: the loss of srl_a2c_grad instead of PPO2's (stage 2 only; no advantage statistics, no clip ratio, no value clip)
-template <int MD, bool A2C>
+// A2C_LOSS: the loss of srl_a2c_grad instead of PPO2's (stage 2 only; no advantage statistics, no clip ratio, no value clip).
+// DQN_LOSS: srl_dqn_grad's dueling Q loss (stage 2) and ReLU instead of tanh (forward, and its derivative in stages 3 and 4).
+template <int MD, int L>
 __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     constexpr bool WIDE = MD != MAXD;
     constexpr int W1S = grad_w1_stride<MD>(), XQ = MD / 4;     // XQ: observation columns per thread of the wide prefetch
@@ -190,7 +205,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     if (t < A) { b3p[t] = a.p.pi_b3[t]; lsd[t] = discrete ? 0.f : a.p.logstd[t]; }
     if (t == 0) b3v[0] = a.p.vf_b3[0];
     __shared__ float s_adv[2];
-    if (!A2C && t < 32) {                  // mean and 1 / (std + 1e-8) (torch.std(): unbiased) from the partial sums, in a fixed order
+    if (L == PPO2_LOSS && t < 32) {                  // mean and 1 / (std + 1e-8) (torch.std(): unbiased) from the partial sums, in a fixed order
         double s1 = a.stats[2 * t] + a.stats[2 * (t + 32)], s2 = a.stats[2 * t + 1] + a.stats[2 * (t + 32) + 1];
         for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(0xffffffffu, s1, o); s2 += __shfl_xor_sync(0xffffffffu, s2, o); }
         if (t == 0) {
@@ -200,7 +215,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
         }
     }
     __syncthreads();
-    const float amean = A2C ? 0.f : s_adv[0], ainv = A2C ? 0.f : s_adv[1], inv_mb = 1.0f / (float)a.mb;
+    const float amean = L != PPO2_LOSS ? 0.f : s_adv[0], ainv = L != PPO2_LOSS ? 0.f : s_adv[1], inv_mb = 1.0f / (float)a.mb;
     // ---- gradient accumulators (registers; every entry of the flat gradient has exactly one owner thread) ----
     const int eg = t >> 4, og = t & 15;          // forward / delta tiles: samples 4 eg + e, units og + 16 k
     const bool own_pi = t < 128;                 // W2 gradient: threads 0..127 own the policy tower's 4 x 8 patches, 128..255 the value tower's
@@ -217,7 +232,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     const int nchunks = (a.mb + CH - 1) / CH;
     SampleRegs cur;
     float xr[XQ];                                // wide: this thread's columns t % 4 + 4 j of sample t / 4 of the next chunk
-    if (t < CH) load_sample<!WIDE, A2C>(a, blockIdx.x * CH + t, cur);
+    if (t < CH) load_sample<!WIDE, L>(a, blockIdx.x * CH + t, cur);
     if constexpr (WIDE) load_row_part<XQ>(a, blockIdx.x * CH + (t >> 2), t & 3, xr);
     __syncthreads();
     for (int c = blockIdx.x; c < nchunks; c += gridDim.x) {
@@ -231,7 +246,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
             for (int k = 0; k < MAXO; ++k) saf[t * MAXO + k] = cur.af[k];
             ssc[t * 4] = cur.adv; ssc[t * 4 + 1] = cur.ret; ssc[t * 4 + 2] = cur.olp; ssc[t * 4 + 3] = cur.ov;
             sai[t * 2] = cur.ai; sai[t * 2 + 1] = cur.valid;
-            load_sample<!WIDE, A2C>(a, (c + gridDim.x) * CH + t, cur);
+            load_sample<!WIDE, L>(a, (c + gridDim.x) * CH + t, cur);
         }
         if constexpr (WIDE) {
 #pragma unroll
@@ -260,7 +275,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
 #pragma unroll
             for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { hap[(4 * eg + e) * WS + og + 16 * k] = tanhf(accp[e][k]); hav[(4 * eg + e) * WS + og + 16 * k] = tanhf(accv[e][k]); }
+                for (int k = 0; k < 4; ++k) { hap[(4 * eg + e) * WS + og + 16 * k] = act_fn<L>(accp[e][k]); hav[(4 * eg + e) * WS + og + 16 * k] = act_fn<L>(accv[e][k]); }
         }
         __syncthreads();
         {
@@ -269,12 +284,12 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
 #pragma unroll
             for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) hbp[(4 * eg + e) * WS + og + 16 * k] = tanhf(o[e][k]);
+                for (int k = 0; k < 4; ++k) hbp[(4 * eg + e) * WS + og + 16 * k] = act_fn<L>(o[e][k]);
             tile_matvec(w2v, b2v, hav, eg, og, o);
 #pragma unroll
             for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) hbv[(4 * eg + e) * WS + og + 16 * k] = tanhf(o[e][k]);
+                for (int k = 0; k < 4; ++k) hbv[(4 * eg + e) * WS + og + 16 * k] = act_fn<L>(o[e][k]);
         }
         __syncthreads();
         {   // heads: thread t -> sample t / 4; outputs t % 4 and t % 4 + 4 of the policy head, the value by lane 3 of the sample's four
@@ -285,7 +300,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
         __syncthreads();
         // ---- 2: d loss / d outputs, one thread per sample ----
         if (t < CH) {
-            const int n = t;
+            const int n = t, row0 = c * CH;            // row0: the chunk's first sample (`c` is the clip range below)
             float z[MAXO], g[MAXO];
 #pragma unroll
             for (int k = 0; k < MAXO; ++k) { z[k] = k < A ? zo[n * (MAXO + 1) + k] : 0.f; g[k] = 0.f; }
@@ -296,7 +311,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
             float gv = 0.f, gl[MAXO];
 #pragma unroll
             for (int k = 0; k < MAXO; ++k) gl[k] = 0.f;
-            if (valid) {
+            if (valid && L != DQN_LOSS) {
                 float logp;
                 float p[MAXO], lse = 0.f, Hent = 0.f;
                 if (discrete) {
@@ -324,7 +339,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
                     }
                 }
                 float dlogp;
-                if constexpr (A2C) {
+                if constexpr (L == A2C_LOSS) {
                     dlogp = -(R - ov) * inv_mb;                                         // pg_loss = mean(-(R - V) logp)
                 } else {
                     const float ratio = expf(logp - olp);
@@ -346,7 +361,7 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
                         gl[k] = dlogp * (p[k] * p[k] - 1.0f) - a.ent_coef * inv_mb;     // d logp / d logstd; entropy = sum(logstd) + const
                     }
                 }
-                if constexpr (A2C) {
+                if constexpr (L == A2C_LOSS) {
                     gv = v - R;                                                         // vf_loss = 0.5 mean((v - R)^2)
                 } else {
                     const float dv = v - ov, dvc = fminf(fmaxf(dv, -c), c);
@@ -355,6 +370,21 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
                     gv = (dvc == dv || l1 > l2) ? e1 : (l1 == l2 ? 0.5f * e1 : 0.f);
                 }
                 gv *= a.vf_coef * inv_mb;
+            }
+            if constexpr (L == DQN_LOSS) {          // Q = V + A - mean(A), td = Q(s, a) - y, loss = mean(w huber(td)), huber with delta = 1
+                if (valid) {
+                    const int ai = sai[n * 2];
+                    float sa = 0.f, za = 0.f;
+#pragma unroll
+                    for (int k = 0; k < MAXO; ++k) if (k < A) { sa += z[k]; if (k == ai) za = z[k]; }
+                    const float inv_a = 1.0f / (float)A;
+                    const float td = (v + (za - sa * inv_a)) - R;
+                    a.td[row0 + n] = td;
+                    const float gq = ov * fminf(fmaxf(td, -1.0f), 1.0f) * inv_mb;      // d loss / d Q(s, a)
+#pragma unroll
+                    for (int k = 0; k < MAXO; ++k) if (k < A) g[k] = gq * ((k == ai ? 1.f : 0.f) - inv_a);
+                    gv = gq;
+                }
             }
 #pragma unroll
             for (int k = 0; k < MAXO; ++k) { d3[n * (MAXO + 1) + k] = g[k]; dls[n * MAXO + k] = gl[k]; }
@@ -377,8 +407,8 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
 #pragma unroll
                     for (int k = 0; k < MAXO; ++k) if (k < A) s = fmaf(w3p[k * WS + j], gz[k], s);
                     const float hp = hbp[n * WS + j], hv = hbv[n * WS + j];
-                    d2p[n * WS + j] = s * (1.0f - hp * hp);
-                    d2v[n * WS + j] = w3v[j] * gvn * (1.0f - hv * hv);
+                    d2p[n * WS + j] = dact_fn<L>(s, hp);
+                    d2v[n * WS + j] = dact_fn<L>(w3v[j] * gvn, hv);
                 }
             }
         }
@@ -439,12 +469,12 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
 #pragma unroll
             for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { const float h = hap[(4 * eg + e) * WS + og + 16 * k]; d1p[(4 * eg + e) * WS + og + 16 * k] = o[e][k] * (1.0f - h * h); }
+                for (int k = 0; k < 4; ++k) { const float h = hap[(4 * eg + e) * WS + og + 16 * k]; d1p[(4 * eg + e) * WS + og + 16 * k] = dact_fn<L>(o[e][k], h); }
             tile_matvec(w2vT, nullptr, d2v, eg, og, o);
 #pragma unroll
             for (int e = 0; e < 4; ++e)
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { const float h = hav[(4 * eg + e) * WS + og + 16 * k]; d1v[(4 * eg + e) * WS + og + 16 * k] = o[e][k] * (1.0f - h * h); }
+                for (int k = 0; k < 4; ++k) { const float h = hav[(4 * eg + e) * WS + og + 16 * k]; d1v[(4 * eg + e) * WS + og + 16 * k] = dact_fn<L>(o[e][k], h); }
         }
         __syncthreads();
         // ---- 5: gradients of layer 1 ----
@@ -501,10 +531,12 @@ __device__ __forceinline__ void ppo2_grad_cta(const GradArgs& a) {
     if (!discrete && t >= 16 && t < 16 + A) out[seg.ls + (t - 16)] = gls;
 }
 
-__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, false>(a); }
-__global__ void __launch_bounds__(NT, 1) ppo2_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, false>(a); }
-__global__ void __launch_bounds__(NT, 1) a2c_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, true>(a); }
-__global__ void __launch_bounds__(NT, 1) a2c_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, true>(a); }
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, PPO2_LOSS>(a); }
+__global__ void __launch_bounds__(NT, 1) ppo2_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, PPO2_LOSS>(a); }
+__global__ void __launch_bounds__(NT, 1) a2c_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, A2C_LOSS>(a); }
+__global__ void __launch_bounds__(NT, 1) a2c_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, A2C_LOSS>(a); }
+__global__ void __launch_bounds__(NT, 1) dqn_grad_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<MAXD, DQN_LOSS>(a); }
+__global__ void __launch_bounds__(NT, 1) dqn_grad_wide_kernel(const __grid_constant__ GradArgs a) { ppo2_grad_cta<WIDE_D, DQN_LOSS>(a); }
 
 // GAE(lambda) of one rollout, the reference's backward recursion (stable-baselines PPO2 runner): one thread per env, T sequential steps,
 // eight steps' loads in flight.  Separate roundings (no FMA contraction): the same bits as the torch recursion of rl_baselines/ppo2.py.
@@ -598,6 +630,51 @@ __global__ void __launch_bounds__(OPT_NT, 1) clip_rmsprop_kernel(const __grid_co
         *msp = ms;
         *wp = __fsub_rn(*wp, __fdiv_rn(__fmul_rn(g, lr), __fsqrt_rn(__fadd_rn(ms, o.eps))));          // w -= g lr / sqrt(ms + eps)
     }
+}
+
+// Per-tensor `tf.clip_by_norm(g, clip_norm)` then one TF1 `AdamOptimizer` step over every tensor of the policy (include/srl_policy.h:
+// srl_clip_adam).  One CTA, like clip_rmsprop_kernel: each tensor's squared norm is summed in float64 in a fixed order; the update keeps the
+// expression order of TF's ApplyAdam with separate float32 roundings, the order rl_baselines/deepq.py's torch restatement evaluates.
+constexpr int NSEG = 13;
+struct AdamArgs { srl_mlp_grads p, g, m, v; Seg seg; const float* lr; float* beta_power; float clip_norm, beta1, beta2, eps; };
+
+__global__ void __launch_bounds__(OPT_NT, 1) clip_adam_kernel(const __grid_constant__ AdamArgs o) {
+    __shared__ double red[OPT_NT / 32];
+    __shared__ float s_norm[NSEG];
+    const int t = threadIdx.x;
+    const Seg& q = o.seg;
+    const int off[NSEG + 1] = {q.pw1, q.pb1, q.pw2, q.pb2, q.pw3, q.pb3, q.vw1, q.vb1, q.vw2, q.vb2, q.vw3, q.vb3, q.ls, q.P};
+    for (int k = 0; k < NSEG; ++k) {
+        double s = 0.0;
+        for (int e = off[k] + t; e < off[k + 1]; e += OPT_NT) { const double g = (double)*seg_elem(o.g, q, e); s = fma(g, g, s); }
+        for (int w = 16; w > 0; w >>= 1) s += __shfl_xor_sync(0xffffffffu, s, w);
+        if ((t & 31) == 0) red[t >> 5] = s;
+        __syncthreads();
+        if (t == 0) {
+            double tot = 0.0;
+            for (int w = 0; w < OPT_NT / 32; ++w) tot += red[w];
+            s_norm[k] = (float)sqrt(tot);
+        }
+        __syncthreads();
+    }
+    const float lr = *o.lr, b1p = o.beta_power[0], b2p = o.beta_power[1];
+    const float lr_t = __fdiv_rn(__fmul_rn(lr, __fsqrt_rn(__fsub_rn(1.0f, b2p))), __fsub_rn(1.0f, b1p));   // lr sqrt(1 - beta2^t) / (1 - beta1^t)
+    const float r1 = __fsub_rn(1.0f, o.beta1), r2 = __fsub_rn(1.0f, o.beta2);
+    for (int e = t; e < q.P; e += OPT_NT) {
+        int k = 0;
+        while (e >= off[k + 1]) ++k;
+        const float nk = s_norm[k];
+        const float den = nk != nk ? nk : fmaxf(nk, o.clip_norm);                          // max(norm, clip_norm), NaN for a NaN norm
+        const float g = __fdiv_rn(__fmul_rn(*seg_elem(o.g, q, e), o.clip_norm), den);       // t clip_norm / max(l2norm, clip_norm)
+        float* mp = seg_elem(o.m, q, e);
+        float* vp = seg_elem(o.v, q, e);
+        float* wp = seg_elem(o.p, q, e);
+        const float m = __fadd_rn(*mp, __fmul_rn(__fsub_rn(g, *mp), r1));                    // m += (g - m) (1 - beta1)
+        const float v = __fadd_rn(*vp, __fmul_rn(__fsub_rn(__fmul_rn(g, g), *vp), r2));      // v += (g^2 - v) (1 - beta2)
+        *mp = m; *vp = v;
+        *wp = __fsub_rn(*wp, __fdiv_rn(__fmul_rn(m, lr_t), __fadd_rn(__fsqrt_rn(v), o.eps)));   // w -= m lr_t / (sqrt(v) + eps)
+    }
+    if (t == 0) { o.beta_power[0] = __fmul_rn(b1p, o.beta1); o.beta_power[1] = __fmul_rn(b2p, o.beta2); }   // TF's beta1_power *= beta1 after the step
 }
 
 template <int MD>
@@ -707,6 +784,43 @@ int srl_a2c_grad(const srl_mlp_policy* p, const srl_mlp_grads* grads, int rows, 
     a.p = *p; a.mb = rows; a.idx = reinterpret_cast<const long long*>(idx); a.obs = obs; a.act = actions; a.ret = ret; a.old_val = old_value;
     a.ent_coef = ent_coef; a.vf_coef = vf_coef; a.partial = reinterpret_cast<float*>(workspace);
     return launch_grad<a2c_grad_kernel, a2c_grad_wide_kernel>(a, grads, ctas, (cudaStream_t)stream);
+}
+
+int srl_dqn_grad(const srl_mlp_policy* q, const srl_mlp_grads* grads, int batch, const int64_t* idx, const float* obs, const int64_t* actions,
+                 const float* y, const float* weights, float* td_out, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!q || !grads || !obs || !actions || !y || !td_out || !workspace) { srl_set_error("dqn_grad: null argument"); return 1; }
+    if (q->struct_size == sizeof(srl_mlp_policy) && !q->discrete) { srl_set_error("dqn_grad: the Q network needs discrete = 1"); return 1; }
+    const int ctas = grad_args_ok("dqn_grad", q, grads, batch);
+    if (ctas <= 0) return 1;
+    const Seg seg = make_seg(q->obs_dim, q->n_out, 1);
+    if (workspace_bytes < sizeof(float) * (size_t)seg.P * (size_t)ctas) { srl_set_error("dqn_grad: workspace too small (srl_a2c_workspace_bytes)"); return 1; }
+    GradArgs a = {};
+    a.p = *q; a.mb = batch; a.idx = reinterpret_cast<const long long*>(idx); a.obs = obs; a.act = actions; a.ret = y; a.old_val = weights;
+    a.partial = reinterpret_cast<float*>(workspace); a.td = td_out;
+    return launch_grad<dqn_grad_kernel, dqn_grad_wide_kernel>(a, grads, ctas, (cudaStream_t)stream);
+}
+
+int srl_clip_adam(int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, const srl_mlp_grads* grads, const srl_mlp_grads* m,
+                  const srl_mlp_grads* v, const float* lr, float* beta_power, float clip_norm, float beta1, float beta2, float epsilon, void* stream) {
+    if (!params || !grads || !m || !v || !lr || !beta_power) { srl_set_error("clip_adam: null argument"); return 1; }
+    if (!discrete) { srl_set_error("clip_adam: the DQN optimiser step takes a discrete Q network (discrete = 1)"); return 1; }
+    if (obs_dim < 1 || obs_dim > WIDE_D || n_out < 1 || n_out > MAXO || (discrete && n_out < 2)) {
+        srl_set_error("clip_adam: unsupported shape obs_dim=%d n_out=%d (obs_dim 1..%d, n_out 1..%d)", obs_dim, n_out, WIDE_D, MAXO); return 1;
+    }
+    if (!(clip_norm > 0.f) || !(beta1 >= 0.f && beta1 < 1.f) || !(beta2 >= 0.f && beta2 < 1.f) || !(epsilon >= 0.f)) {
+        srl_set_error("clip_adam: need clip_norm > 0, 0 <= beta1, beta2 < 1, epsilon >= 0 (got %g, %g, %g, %g)", clip_norm, beta1, beta2, epsilon); return 1;
+    }
+    for (const srl_mlp_grads* t : {params, grads, m, v}) {
+        if (t->struct_size != sizeof(srl_mlp_grads)) { srl_set_error("clip_adam: struct size mismatch"); return 1; }
+        if (!t->pi_w1 || !t->pi_b1 || !t->pi_w2 || !t->pi_b2 || !t->pi_w3 || !t->pi_b3 || !t->vf_w1 || !t->vf_b1 || !t->vf_w2 || !t->vf_b2 || !t->vf_w3 ||
+            !t->vf_b3 || (!discrete && !t->logstd)) { srl_set_error("clip_adam: null tensor pointer"); return 1; }
+    }
+    AdamArgs o;
+    o.p = *params; o.g = *grads; o.m = *m; o.v = *v; o.seg = make_seg(obs_dim, n_out, discrete); o.lr = lr; o.beta_power = beta_power;
+    o.clip_norm = clip_norm; o.beta1 = beta1; o.beta2 = beta2; o.eps = epsilon;
+    clip_adam_kernel<<<1, OPT_NT, 0, (cudaStream_t)stream>>>(o);
+    SRL_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 int srl_clip_rmsprop(int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, const srl_mlp_grads* grads, const srl_mlp_grads* ms,

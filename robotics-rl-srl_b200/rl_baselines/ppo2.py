@@ -133,10 +133,11 @@ def allreduce_mean_gradients(params, dist, world):
 # ---- pieces shared with rl_baselines/a2c.py: the run's envs, policy and first observation, the collection loop, and the per-update
 #      bookkeeping (monitor log, episode statistics, best-model callback, saved model and run files) ----
 
-def make_run(algo, env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, fused_flags):
+def make_run(algo, env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, fused_flags, network=None):
     """The envs of this process (global env offset ``rank * num_envs``) and a policy over rows of ``num_stack * D`` values, identical on
     every rank.  ``fused_flags``: the trainer's fused-path switches (None: on whenever the envs live on a GPU); rows wider than the fused
-    kernels take are refused when any is on.  Call after ``torch.manual_seed(seed)``; reseeds with ``seed + rank`` when data-parallel."""
+    kernels take are refused when any is on.  ``network(width, env)``: builds another network than the MlpPolicy (rl_baselines/deepq.py's Q
+    network); it becomes ``run.policy``.  Call after ``torch.manual_seed(seed)``; reseeds with ``seed + rank`` when data-parallel."""
     env_kwargs = dict(env_kwargs or {})
     dist, rank, world = _dist_world()
     if prefetch_resets is None:
@@ -164,7 +165,9 @@ def make_run(algo, env_id, num_envs, seed, env_kwargs, device, prefetch_resets, 
     if W > 32 and any(on_gpu if f is None else f for f in fused_flags):
         from srl_sim.policy import MAX_OBS
         raise ValueError("num_stack=%d x %d-wide observations = %d: the fused policy kernels take at most %d values per row" % (K, D, W, MAX_OBS))
-    if env.is_discrete:
+    if network is not None:
+        policy = network(W, env).to(dev)
+    elif env.is_discrete:
         policy = MlpPolicy(W, n_actions=env.action_space.n).to(dev)
     else:
         policy = MlpPolicy(W, action_dim=env.action_space.shape[0]).to(dev)

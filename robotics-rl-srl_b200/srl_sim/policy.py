@@ -9,11 +9,12 @@ Reference pieces replaced: stable-baselines' ``PPO2`` runner ``model.step(obs)``
 There is no CPU fallback here either: :class:`FusedPolicy` needs the CUDA library and CUDA tensors.
 """
 import ctypes
-from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32, c_size_t, c_uint32, c_uint64, c_void_p
+from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint32, c_uint64, c_void_p
 
 HIDDEN, MAX_OBS, MAX_OUT = 64, 32, 8     # observation widths 1..8 and 9..32 (stacked states) run separate kernel instantiations
 POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae",
-                  "srl_a2c_grad", "srl_a2c_workspace_bytes", "srl_clip_rmsprop"]
+                  "srl_a2c_grad", "srl_a2c_workspace_bytes", "srl_clip_rmsprop", "srl_dqn_act", "srl_dqn_target", "srl_dqn_grad", "srl_clip_adam",
+                  "srl_replay_add", "srl_replay_sample", "srl_replay_update"]
 GRAD_NAMES = ["pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3", "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3", "logstd"]
 
 
@@ -29,6 +30,12 @@ class SrlMlpGrads(Structure):
     _fields_ = [("struct_size", c_uint32), ("reserved", c_uint32)] + \
                [(name, c_void_p) for name in ("pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3",
                                               "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3", "logstd")]
+
+
+class SrlReplayTree(Structure):
+    """struct srl_replay_tree (include/srl_policy.h)."""
+    _fields_ = [("struct_size", c_uint32), ("n_envs", c_int32), ("capacity", c_int64), ("tree_cap", c_int64)] + \
+               [(name, c_void_p) for name in ("sum", "min", "max_priority", "size", "stamp")]
 
 
 def bind(cdll):
@@ -54,6 +61,22 @@ def bind(cdll):
     cdll.srl_clip_rmsprop.restype = c_int
     cdll.srl_clip_rmsprop.argtypes = [c_int, c_int, c_int, POINTER(SrlMlpGrads), POINTER(SrlMlpGrads), POINTER(SrlMlpGrads), c_void_p, c_float, c_float,
                                       c_float, c_void_p]
+    P, G = POINTER(SrlMlpPolicy), POINTER(SrlMlpGrads)
+    cdll.srl_dqn_act.restype = c_int
+    cdll.srl_dqn_act.argtypes = [P, c_int, c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    cdll.srl_dqn_target.restype = c_int
+    cdll.srl_dqn_target.argtypes = [P, P, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p]
+    cdll.srl_dqn_grad.restype = c_int
+    cdll.srl_dqn_grad.argtypes = [P, G, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_clip_adam.restype = c_int
+    cdll.srl_clip_adam.argtypes = [c_int, c_int, c_int, G, G, G, G, c_void_p, c_void_p, c_float, c_float, c_float, c_float, c_void_p]
+    T = POINTER(SrlReplayTree)
+    cdll.srl_replay_add.restype = c_int
+    cdll.srl_replay_add.argtypes = [T, c_int64, c_double, c_void_p]
+    cdll.srl_replay_sample.restype = c_int
+    cdll.srl_replay_sample.argtypes = [T, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    cdll.srl_replay_update.restype = c_int
+    cdll.srl_replay_update.argtypes = [T, c_int, c_void_p, c_void_p, c_double, c_float, c_void_p]
     return cdll
 
 
@@ -228,3 +251,136 @@ class FusedClipRMSprop(object):
         rc = self._lib.srl_clip_rmsprop(self.obs_dim, self.n_out, self.discrete, byref(self._p), byref(self._g), byref(self._m), lr.data_ptr(),
                                         self.max_grad_norm, self.alpha, self.epsilon, stream)
         self._library.check(rc, "srl_clip_rmsprop")
+
+
+# ---- DQN (include/srl_policy.h: srl_dqn_*, srl_replay_*, srl_clip_adam; rl_baselines/deepq.py) ----
+
+def _cuda_policy_struct(lib_name, policy):
+    st, keep = policy_struct(policy)
+    if policy.pi[0].weight.device.type != "cuda":
+        raise ValueError("%s needs a network on a CUDA device (there is no CPU fallback)" % lib_name)
+    if not st.discrete:
+        raise ValueError("%s: the Q network must be discrete" % lib_name)
+    return st, keep
+
+
+class FusedDQNAct(object):
+    """``srl_dqn_act``: the epsilon-greedy step of a dueling Q network (``rl_baselines.deepq.DuelingQ``) for one env batch, in one launch.
+    Owns the sampling record ``rng`` {seed, counter, 0} and the exploration rate ``eps`` (float32 [1] on the device)."""
+
+    def __init__(self, library, qnet, seed, env_offset=0):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        self.struct, self._keep = _cuda_policy_struct("FusedDQNAct", qnet)
+        dev = qnet.pi[0].weight.device
+        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=dev)
+        self.eps = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.env_offset = int(env_offset)
+
+    def __call__(self, n, obs, act_env, obs_buf=None, act_buf=None, q_out=None, eps=None, stream=None):
+        """``eps``: a float32 device scalar to read the exploration rate from (default: this object's ``eps``)."""
+        ptr = lambda t: None if t is None else t.data_ptr()
+        rc = self._lib.srl_dqn_act(byref(self.struct), int(n), obs.data_ptr(), (self.eps if eps is None else eps).data_ptr(), self.rng.data_ptr(), self.env_offset, ptr(obs_buf),
+                                   act_env.data_ptr(), ptr(act_buf), ptr(q_out), stream)
+        self._library.check(rc, "srl_dqn_act")
+
+
+class FusedDQNTarget(object):
+    """``srl_dqn_target``: the double-Q targets ``y`` of a sampled batch from the online and the target network (both live tensors)."""
+
+    def __init__(self, library, online, target):
+        self._lib = bind(library.lib)
+        self._library = library
+        self.online, self._keep_o = _cuda_policy_struct("FusedDQNTarget", online)
+        self.target, self._keep_t = _cuda_policy_struct("FusedDQNTarget", target)
+
+    def __call__(self, batch, idx, next_obs, rew, done, gamma, y, stream=None):
+        rc = self._lib.srl_dqn_target(byref(self.online), byref(self.target), int(batch), None if idx is None else idx.data_ptr(), next_obs.data_ptr(),
+                                      rew.data_ptr(), done.data_ptr(), float(gamma), y.data_ptr(), stream)
+        self._library.check(rc, "srl_dqn_target")
+
+
+class FusedDQNGrad(FusedPPO2Grad):
+    """``srl_dqn_grad``: the gradient of ``mean(w huber(Q(s, a) - y))`` over a batch of ``minibatch`` samples, in the kernels of
+    :class:`FusedPPO2Grad`, into the network's static ``.grad`` tensors; also writes the per-sample td."""
+    _workspace_fn = "srl_a2c_workspace_bytes"
+
+    def __call__(self, idx, obs, actions, y, weights, td_out, stream=None):
+        rc = self._lib.srl_dqn_grad(byref(self.struct), byref(self.grads), self.minibatch, None if idx is None else idx.data_ptr(), obs.data_ptr(),
+                                    actions.data_ptr(), y.data_ptr(), None if weights is None else weights.data_ptr(), td_out.data_ptr(),
+                                    self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._library.check(rc, "srl_dqn_grad")
+
+
+class FusedClipAdam(object):
+    """``srl_clip_adam``: ``tf.clip_by_norm`` per tensor + one TF1 Adam step over every tensor of the network in one launch.  Reads the
+    ``.grad`` tensors (static: :class:`FusedDQNGrad` makes them), owns the slots ``m``, ``v`` (zeros), TF's ``beta_power`` accumulators
+    {beta1^t, beta2^t} (float32 [2], from {beta1, beta2}) and the learning rate ``lr`` (float32 [1])."""
+
+    def __init__(self, library, policy, clip_norm, beta1=0.9, beta2=0.999, epsilon=1e-8):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        self.params = policy_params(policy)
+        dev = self.params[0].device
+        if dev.type != "cuda":
+            raise ValueError("FusedClipAdam needs a network on a CUDA device (there is no CPU fallback)")
+        if any(p.grad is None for p in self.params):
+            raise ValueError("FusedClipAdam needs the network's .grad tensors (create them first, e.g. with FusedDQNGrad)")
+        st, _ = policy_struct(policy)
+        self.obs_dim, self.n_out, self.discrete = st.obs_dim, st.n_out, st.discrete
+        self.m = [torch.zeros_like(p) for p in self.params]
+        self.v = [torch.zeros_like(p) for p in self.params]
+        self.beta_power = torch.tensor([beta1, beta2], dtype=torch.float32, device=dev)
+        self.lr = torch.zeros(1, dtype=torch.float32, device=dev)
+        self._p, self._g = tensors_struct(self.params), tensors_struct([p.grad for p in self.params])
+        self._m, self._v = tensors_struct(self.m), tensors_struct(self.v)
+        self.clip_norm, self.beta1, self.beta2, self.epsilon = float(clip_norm), float(beta1), float(beta2), float(epsilon)
+
+    def __call__(self, stream=None):
+        rc = self._lib.srl_clip_adam(self.obs_dim, self.n_out, self.discrete, byref(self._p), byref(self._g), byref(self._m), byref(self._v),
+                                     self.lr.data_ptr(), self.beta_power.data_ptr(), self.clip_norm, self.beta1, self.beta2, self.epsilon, stream)
+        self._library.check(rc, "srl_clip_adam")
+
+
+class FusedReplay(object):
+    """baselines' prioritized replay over a ring of ``rows`` x ``n_envs`` transitions on the device (``srl_replay_*``): the two float64
+    segment trees, ``max_priority``, the stored count ``size``, the sampling record ``rng`` and the importance exponent ``beta`` (float64 [1]).
+    ``sum`` / ``min`` are [2 tree_cap] with the root at 1 and leaf i at tree_cap + i."""
+
+    def __init__(self, library, rows, n_envs, seed, alpha, device):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        capacity = int(rows) * int(n_envs)
+        tree_cap = 1
+        while tree_cap < capacity:
+            tree_cap *= 2
+        self.alpha, self.n_envs, self.capacity, self.tree_cap = float(alpha), int(n_envs), capacity, tree_cap
+        self.sum = torch.zeros(2 * tree_cap, dtype=torch.float64, device=device)
+        self.min = torch.full((2 * tree_cap,), float("inf"), dtype=torch.float64, device=device)
+        self.max_priority = torch.ones(1, dtype=torch.float64, device=device)
+        self.size = torch.zeros(1, dtype=torch.int64, device=device)
+        self.stamp = torch.full((capacity,), -1, dtype=torch.int32, device=device)
+        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=device)
+        self.beta = torch.zeros(1, dtype=torch.float64, device=device)
+        t = SrlReplayTree()
+        t.struct_size = ctypes.sizeof(SrlReplayTree)
+        t.n_envs, t.capacity, t.tree_cap = self.n_envs, capacity, tree_cap
+        for name in ("sum", "min", "max_priority", "size", "stamp"):
+            setattr(t, name, getattr(self, name).data_ptr())
+        self.struct = t
+
+    def add(self, row, stream=None):
+        self._library.check(self._lib.srl_replay_add(byref(self.struct), int(row), self.alpha, stream), "srl_replay_add")
+
+    def sample(self, batch, idx_out, w_out, prioritized=True, beta=None, stream=None):
+        """``beta``: a float64 device scalar to read the importance exponent from (default: this object's ``beta``)."""
+        rc = self._lib.srl_replay_sample(byref(self.struct), int(batch), int(bool(prioritized)), (self.beta if beta is None else beta).data_ptr(), self.rng.data_ptr(),
+                                         idx_out.data_ptr(), w_out.data_ptr(), stream)
+        self._library.check(rc, "srl_replay_sample")
+
+    def update(self, batch, idx, td, eps, stream=None):
+        rc = self._lib.srl_replay_update(byref(self.struct), int(batch), idx.data_ptr(), td.data_ptr(), self.alpha, float(eps), stream)
+        self._library.check(rc, "srl_replay_update")
