@@ -385,5 +385,6 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     env.close()
     train.best_mean_reward, train.n_saved, train.stats = log.best_mean_reward, log.n_saved, stats
     train.last_policy, train.last_target, train.last_norm, train.last_replay = qnet, target, norm, replay
+    train.last_ring = ring
     train.last_adam = (m, v, beta_power)
     return log.history

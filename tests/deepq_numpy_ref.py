@@ -6,6 +6,8 @@ srl_clip_adam) and not from rl_baselines/deepq.py, for the CPU and GPU tests of 
   double_q_model      : y = r + gamma (1 - d) Q_target(s', argmax Q_online(s'))
   clip_adam_model     : tf.clip_by_norm per tensor followed by TF1 Adam, on lists of arrays
   SegmentTree / PrioritizedReplay : a direct transcription of baselines' SegmentTree (loop form) and of the prioritized buffer's bookkeeping
+  first_sample_model  : the indices of a replay's first batch, while every stored leaf is still 1^alpha (uniform or prioritized)
+  dqn_step_model      : one gradient step from zero Adam slots (double Q with one network as online and target, gradient, clip, Adam)
 """
 import operator
 
@@ -149,3 +151,34 @@ class PrioritizedReplay(object):
 
     def trees(self):
         return np.array(self.it_sum._value), np.array(self.it_min._value)
+
+
+def first_sample_model(u, n, tree_cap, prioritized, boundary=1e-11):
+    """Indices of the uniforms ``u`` over ``n`` stored transitions whose leaves all hold 1 (a tree of ``tree_cap`` leaves, zeros past n),
+    and the samples whose index may differ by one in a float64 walk (``u n`` within ``boundary n`` of a leaf boundary: the rule of the
+    replay tests).  Uniform: min(floor(u n), n - 1), exact.  Prioritized: find_prefixsum_idx walked without building the tree, a node's sum
+    being the number of stored leaves under it, and a walk into an empty leaf clamped to n - 1."""
+    u = np.asarray(u, np.float64)
+    if not prioritized:
+        return np.minimum((u * n).astype(np.int64), n - 1), np.zeros(len(u), bool)
+    mass, node, span = u * float(n), np.ones(len(u), np.int64), int(tree_cap)
+    while span > 1:
+        span //= 2
+        left = np.clip(n - (2 * node * span - tree_cap), 0, span).astype(np.float64)      # stored leaves under the left child
+        go_left = left > mass
+        mass = np.where(go_left, mass, mass - left)
+        node = 2 * node + (~go_left)
+    un = u * float(n)
+    return np.minimum(node - tree_cap, n - 1), np.abs(un - np.round(un)) <= boundary * n
+
+
+def dqn_step_model(qnet, obs, act, rew, done, next_obs, gamma, lr, clip_norm, beta1, beta2, eps):
+    """One gradient step of a DQN whose online and target networks are both ``qnet`` and whose Adam slots are zero, over sampled rows with
+    importance weights 1: y (double Q), td and the gradients, the per-tensor clip factors, and the parameters and slots after the step."""
+    y, _ = double_q_model(qnet, qnet, rew, done, next_obs, gamma)
+    grads, td = dqn_grads_model(qnet, obs, act, y, np.ones(len(y)))
+    params = [p.detach().cpu().double().numpy() for p in qnet.parameters()]
+    new, m, v = clip_adam_model(params, grads, [np.zeros(p.shape) for p in params], [np.zeros(p.shape) for p in params], 1, lr, clip_norm,
+                                beta1, beta2, eps)
+    scale = [clip_norm / max(np.sqrt((g * g).sum()), clip_norm) for g in grads]
+    return dict(y=y, td=td, grads=grads, clip_scale=scale, params=params, new_params=new, m=m, v=v)

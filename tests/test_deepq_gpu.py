@@ -1,13 +1,16 @@
 """
 GPU tests of the DQN path (include/srl_policy.h: srl_dqn_*, srl_replay_*, srl_clip_adam; rl_baselines/deepq.py):
-  srl_dqn_act       -- Q against float64, greedy actions at epsilon 0, the exploration rate and uniformity (chi-square), the same bytes twice;
+  srl_dqn_act       -- Q against float64, greedy actions at epsilon 0, the exploration rate and uniformity (chi-square), the same bytes twice,
+                       two sharded launches (env_offset) give the bytes of one, successive launches draw successive counters;
   srl_replay_*      -- the trees, indices and weights against the loop-form transcription of baselines' SegmentTree (tests/deepq_numpy_ref.py)
-                       fed the kernel's own Philox uniforms, and at the trainer's 4096 x 1000 against the vectorised tree of rl_baselines.deepq;
-  srl_dqn_target    -- y against float64 double Q;
+                       fed the kernel's own Philox uniforms, and at the trainer's 4096 x 1000 and 8192 x 1000 (two and three rebuild passes)
+                       against the vectorised tree of rl_baselines.deepq; prioritized and uniform sampling;
+  srl_dqn_target    -- y against float64 double Q, with one chunk and several chunks per CTA, through idx and without;
   srl_dqn_grad      -- float64 autograd of rl_baselines.deepq.dqn_loss with the tolerance rule of tests/test_consumer_kernels_gpu.py, the same
-                       bytes twice, and shown to see a missing row;
+                       bytes twice, no weights (NULL) as all-ones weights, and shown to see a missing row;
   srl_clip_adam     -- the float64 TF model over 100 steps, the same bytes twice, non-finite gradients;
   the trainer       -- learns MobileRobot, captured and eager runs give the same bytes, and the entry point runs for every env id.
+One whole gradient step of the trainer against float64: tests/test_deepq_step_gpu.py.
 """
 import copy
 
@@ -107,8 +110,38 @@ def test_dqn_act_explores_at_the_rate_epsilon_uniformly(cuda_lib, philox_u53):
     assert np.array_equal(runs[1], runs[2])
 
 
-def _replay_run(cuda_lib, philox_u53, rows, N, B, n_adds, seed=9, check_loop=True):
-    """Adds (wrapping the ring), then rounds of sample + update with the kernels, mirrored step by step on the numpy statements."""
+def test_dqn_act_sharded_launches_and_successive_counters(cuda_lib, philox_u53):
+    """Envs [0, k) and [k, n) in two launches, the second with env_offset = k (k odd, inside a CTA of 32 envs), as data-parallel ranks launch:
+    the actions and Q bytes of one launch over [0, n).  Three successive launches draw with counters 0, 1 and 2."""
+    from srl_sim.policy import FusedDQNAct
+    n, k, A, seed = 1000, 45, 6, 13
+    q = _qnet(3, A)
+    obs = torch.randn(n, 3, device="cuda")
+
+    def launch(f, lo, hi, eps):
+        act, qout = torch.zeros(hi - lo, dtype=torch.int32, device="cuda"), torch.zeros(hi - lo, A, device="cuda")
+        f.eps.fill_(eps)
+        f(hi - lo, obs[lo:hi], act, q_out=qout, stream=_stream())
+        torch.cuda.synchronize()
+        return act, qout
+    whole = launch(FusedDQNAct(cuda_lib, q, seed=seed), 0, n, 0.5)
+    parts = [launch(FusedDQNAct(cuda_lib, q, seed=seed, env_offset=lo), lo, hi, 0.5) for lo, hi in ((0, k), (k, n))]
+    assert torch.equal(torch.cat([p[0] for p in parts]), whole[0]) and torch.equal(torch.cat([p[1] for p in parts]), whole[1])
+    greedy = launch(FusedDQNAct(cuda_lib, q, seed=seed), 0, n, 0.0)[0].cpu().numpy()
+    f, explored = FusedDQNAct(cuda_lib, q, seed=seed), []
+    for counter in range(3):
+        act = launch(f, 0, n, 0.5)[0].cpu().numpy()
+        assert int(f.rng[1]) == counter + 1
+        u, w2 = philox_u53(seed, range(n), counter, PURPOSE_ACT)
+        explore = u < 0.5
+        assert np.array_equal(act[explore], ((w2[explore] * A) >> 32).astype(np.int64)) and np.array_equal(act[~explore], greedy[~explore])
+        explored.append(explore)
+    assert not np.array_equal(explored[0], explored[1]) and not np.array_equal(explored[1], explored[2])
+
+
+def _replay_run(cuda_lib, philox_u53, rows, N, B, n_adds, seed=9, check_loop=True, prioritized=True):
+    """Adds (wrapping the ring), then rounds of sample + update with the kernels, mirrored step by step on the numpy statements.  Uniform
+    (``prioritized=False``): rounds of sample only, as the trainer runs them; the indices are exact, the weights 1, the trees untouched."""
     from rl_baselines.deepq import ReplayTree
     from srl_sim.policy import FusedReplay
     rep = FusedReplay(cuda_lib, rows, N, seed, 0.6, "cuda")
@@ -126,33 +159,41 @@ def _replay_run(cuda_lib, philox_u53, rows, N, B, n_adds, seed=9, check_loop=Tru
         if step >= 2:
             beta = 0.4 + 0.05 * step
             rep.beta.fill_(beta)
-            rep.sample(B, idx, w, stream=_stream())
+            trees = (rep.sum.clone(), rep.min.clone(), rep.max_priority.clone(), rep.size.clone())
+            rep.sample(B, idx, w, prioritized=prioritized, stream=_stream())
             torch.cuda.synchronize()
             u, _ = philox_u53(seed, range(B), counter, PURPOSE_REPLAY)
             counter += 1
-            ix, wv = vec.sample(u, beta)
-            got_i, got_w = idx.cpu().numpy(), w.cpu().numpy()
-            # an index may differ only where the mass sits within float64 rounding of the boundary between the two leaves
-            bad = got_i != ix
-            stats["near"] += int(bad.sum())
-            if bad.any():
-                total, cap = vec.sum[1], vec.tree_cap
-                cum = np.cumsum(vec.sum[cap:cap + vec.size])
-                lo = np.minimum(got_i[bad], ix[bad])
-                assert np.all(np.abs(got_i[bad] - ix[bad]) == 1), (got_i[bad], ix[bad])
-                assert np.all(np.abs(u[bad] * total - cum[lo]) <= 1e-11 * total), np.abs(u[bad] * total - cum[lo]).max() / total
-            ok = ~bad
-            assert np.allclose(got_w[ok], wv[ok], rtol=1e-6, atol=0)
-            if loop:
-                li, lw = loop.sample(u, beta)
-                assert np.array_equal(li[ok], ix[ok]) and np.allclose(lw[ok], wv[ok], rtol=1e-6, atol=0)
-            # the batch's td: large and small, with repeated indices
-            td = torch.randn(B, device="cuda", generator=g) * 2.0
-            stats["dup"] += B - len(np.unique(got_i))
-            rep.update(B, idx, td, 1e-6, stream=_stream())
-            vec.update(got_i, td.cpu().numpy(), 1e-6)
-            if loop:
-                loop.update_priorities(got_i, td.cpu().numpy(), 1e-6)
+            assert int(rep.rng[1]) == counter and int(rep.rng[2]) == 0
+            assert all(torch.equal(a, b) for a, b in zip(trees, (rep.sum, rep.min, rep.max_priority, rep.size)))
+            ix, wv = vec.sample(u, beta, prioritized)
+            if not prioritized:                      # min(floor(u n), n - 1) exactly, weights exactly 1
+                assert np.array_equal(idx.cpu().numpy(), np.minimum(np.floor(u * vec.size).astype(np.int64), vec.size - 1))
+                assert bool((w == 1.0).all())
+                stats["dup"] += B - len(np.unique(ix))
+            else:
+                got_i, got_w = idx.cpu().numpy(), w.cpu().numpy()
+                # an index may differ only where the mass sits within float64 rounding of the boundary between the two leaves
+                bad = got_i != ix
+                stats["near"] += int(bad.sum())
+                if bad.any():
+                    total, cap = vec.sum[1], vec.tree_cap
+                    cum = np.cumsum(vec.sum[cap:cap + vec.size])
+                    lo = np.minimum(got_i[bad], ix[bad])
+                    assert np.all(np.abs(got_i[bad] - ix[bad]) == 1), (got_i[bad], ix[bad])
+                    assert np.all(np.abs(u[bad] * total - cum[lo]) <= 1e-11 * total), np.abs(u[bad] * total - cum[lo]).max() / total
+                ok = ~bad
+                assert np.allclose(got_w[ok], wv[ok], rtol=1e-6, atol=0)
+                if loop:
+                    li, lw = loop.sample(u, beta)
+                    assert np.array_equal(li[ok], ix[ok]) and np.allclose(lw[ok], wv[ok], rtol=1e-6, atol=0)
+                # the batch's td: large and small, with repeated indices
+                td = torch.randn(B, device="cuda", generator=g) * 2.0
+                stats["dup"] += B - len(np.unique(got_i))
+                rep.update(B, idx, td, 1e-6, stream=_stream())
+                vec.update(got_i, td.cpu().numpy(), 1e-6)
+                if loop:
+                    loop.update_priorities(got_i, td.cpu().numpy(), 1e-6)
         torch.cuda.synchronize()
         s, m = rep.sum.cpu().numpy(), rep.min.cpu().numpy()
         cap = rep.tree_cap
@@ -161,6 +202,8 @@ def _replay_run(cuda_lib, philox_u53, rows, N, B, n_adds, seed=9, check_loop=Tru
         # every internal node is op(left, right) of the kernel's own nodes, bit for bit
         k = np.arange(1, cap)
         assert np.array_equal(s[k], s[2 * k] + s[2 * k + 1]) and np.array_equal(m[k], np.minimum(m[2 * k], m[2 * k + 1]))
+        # ... up to the root, which holds the float64 sum and the minimum of the leaves
+        assert abs(s[1] - np.sum(s[cap:])) <= 1e-12 * s[1] and m[1] == m[cap:].min()
         assert float(rep.max_priority) == vec.max_priority and int(rep.size) == vec.size
         if loop:
             ls, lm = loop.trees()
@@ -170,40 +213,53 @@ def _replay_run(cuda_lib, philox_u53, rows, N, B, n_adds, seed=9, check_loop=Tru
 
 
 def test_replay_kernels_match_the_segment_tree_transcription(cuda_lib, philox_u53):
-    """A ring of 5 rows x 7 envs (a non-power-of-two capacity, 64 leaves), 12 adds (the ring wraps twice), batches with repeated indices."""
-    stats = _replay_run(cuda_lib, philox_u53, rows=5, N=7, B=50, n_adds=12)
-    assert stats["dup"] > 0
+    """A ring of 5 rows x 7 envs (a non-power-of-two capacity, 64 leaves), 12 adds (the ring wraps twice), batches with repeated indices;
+    prioritized sampling, then uniform sampling."""
+    for prioritized in (True, False):
+        stats = _replay_run(cuda_lib, philox_u53, rows=5, N=7, B=50, n_adds=12, prioritized=prioritized)
+        assert stats["dup"] > 0, prioritized
 
 
 def test_replay_kernels_at_the_trainers_size(cuda_lib, philox_u53):
-    """4096 envs x 1000 rows (4 096 000 transitions, 2^22 leaves), 131 072 samples per batch: the vectorised tree of rl_baselines.deepq."""
-    stats = _replay_run(cuda_lib, philox_u53, rows=1000, N=4096, B=131072, n_adds=4, check_loop=False)
-    print("\nreplay at 4096 x 1000: %d duplicate samples, %d indices on a float64 boundary" % (stats["dup"], stats["near"]))
-    assert stats["dup"] > 0
+    """N envs x 1000 rows, 32 N samples per batch, prioritized then uniform: the vectorised tree of rl_baselines.deepq.  4096 x 1000
+    (4 096 000 transitions) is a tree of 2^22 leaves, rebuilt in two passes (subtrees of 2048 leaves, then the level of their 2048 roots);
+    8192 x 1000 is 2^23 leaves and three passes, each add (8192 leaves) spanning four 2048-leaf subtrees."""
+    for N in (4096, 8192):
+        for prioritized in (True, False):
+            stats = _replay_run(cuda_lib, philox_u53, rows=1000, N=N, B=32 * N, n_adds=4, check_loop=False, prioritized=prioritized)
+            print("\nreplay at %d x 1000 (%s): %d duplicate samples, %d indices on a float64 boundary"
+                  % (N, "prioritized" if prioritized else "uniform", stats["dup"], stats["near"]))
+            assert stats["dup"] > 0, (N, prioritized)
 
 
 @pytest.mark.parametrize("width,n_act", Q_SHAPES)
 def test_dqn_target_matches_float64_double_q(cuda_lib, width, n_act):
+    """Batches of 2049 samples (one chunk of 32 per CTA at most), sms 32 3 + 17 and the trainer's 131 072 (every CTA of the persistent grid
+    walks several chunks), read through idx and straight from the first rows (idx = None)."""
     from srl_sim.policy import FusedDQNTarget
-    rows, B = 3000, 2049
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     online, target = _qnet(width, n_act, seed=1), _qnet(width, n_act, seed=2)
-    g = torch.Generator(device="cuda").manual_seed(4)
-    nxt = torch.randn(rows, width, device="cuda", generator=g)
-    rew = torch.randn(rows, device="cuda", generator=g)
-    done = (torch.rand(rows, device="cuda", generator=g) < 0.2).to(torch.uint8)
-    idx = torch.randint(0, rows, (B,), device="cuda", generator=g)
-    y = torch.zeros(B, device="cuda")
-    FusedDQNTarget(cuda_lib, online, target)(B, idx, nxt, rew, done, 0.99, y, stream=_stream())
-    torch.cuda.synchronize()
-    ix = idx.cpu().numpy()
-    want, qo = double_q_model(online, target, rew.cpu().numpy()[ix], done.cpu().numpy()[ix], nxt.cpu().numpy()[ix], 0.99)
-    got = y.cpu().numpy()
-    tol = 2e-5 * (np.abs(want).max() + 1.0)
-    bad = np.abs(got - want) > tol
-    # a flip of the online argmax is allowed only where its top two are within float32 rounding
-    top2 = np.sort(qo, 1)[:, -2:]
-    assert np.all(top2[bad, 1] - top2[bad, 0] < 1e-4 * (np.abs(qo).max() + 1.0)), (bad.sum(), np.abs(got - want).max())
-    assert bad.sum() <= 2
+    fused = FusedDQNTarget(cuda_lib, online, target)
+    for B in (2049, sms * 32 * 3 + 17, 131072):
+        rows = 3000 if B == 2049 else B + B // 3 + 1
+        g = torch.Generator(device="cuda").manual_seed(4)
+        nxt = torch.randn(rows, width, device="cuda", generator=g)
+        rew = torch.randn(rows, device="cuda", generator=g)
+        done = (torch.rand(rows, device="cuda", generator=g) < 0.2).to(torch.uint8)
+        for idx in (torch.randint(0, rows, (B,), device="cuda", generator=g), None):
+            y = torch.zeros(B, device="cuda")
+            fused(B, idx, nxt, rew, done, 0.99, y, stream=_stream())
+            torch.cuda.synchronize()
+            ix = np.arange(B) if idx is None else idx.cpu().numpy()
+            want, qo = double_q_model(online, target, rew.cpu().numpy()[ix], done.cpu().numpy()[ix], nxt.cpu().numpy()[ix], 0.99)
+            got = y.cpu().numpy()
+            tol = 2e-5 * (np.abs(want).max() + 1.0)
+            bad = np.abs(got - want) > tol
+            # a flip of the online argmax is allowed only where its top two are within float32 rounding
+            top2 = np.sort(qo, 1)[:, -2:]
+            case = (B, "idx" if idx is not None else "no idx", int(bad.sum()), float(np.abs(got - want).max()))
+            assert np.all(top2[bad, 1] - top2[bad, 0] < 1e-4 * (np.abs(qo).max() + 1.0)), case
+            assert bad.sum() <= max(2, B // 1000), case
 
 
 def _away_from_relu_kinks(q, obs, g):
@@ -275,8 +331,25 @@ def test_dqn_grad_matches_float64_autograd(cuda_lib, width, n_act, size, use_idx
         fused(idx, obs, act, y, w, td2, stream=_stream())
         torch.cuda.synchronize()
         assert all(torch.equal(p.grad, a) for p, a in zip(q.parameters(), got)) and torch.equal(td, td2)
+    plain = copy.deepcopy(q)                 # without the kernel's .grad tensors, into which a reference's backward would accumulate
+    for p in plain.parameters():
+        p.grad = None
+    if size in ("33", "3_chunks_per_cta"):
+        # weights = NULL, as the trainer passes without prioritized replay: the bytes of all-ones weights, and float64 autograd with w = 1
+        ones, out = torch.ones(B, device="cuda"), []
+        for wt in (None, ones):
+            fused(idx, obs, act, y, wt, td, stream=_stream())
+            torch.cuda.synchronize()
+            out.append([p.grad.detach().clone() for p in q.parameters()] + [td.clone()])
+        assert all(torch.equal(a, b) for a, b in zip(*out))
+        d1 = dict(d, w=ones)
+        want1, td1 = _dqn_grads(copy.deepcopy(plain).double(), d1, ref_idx)
+        f32_1 = grad_errors(_dqn_grads(plain, d1, ref_idx)[0], want1)
+        for n, (err, scale), (e32, _) in zip(names, grad_errors(out[0][:-1], want1), f32_1):
+            assert scale > 0 and err <= grad_bound(scale) + 4.0 * e32, ("w = None", n, err, e32, scale)
+        assert float((out[0][-1].double() - td1).abs().max()) <= 2e-5 * (float(td1.abs().max()) + 1.0)
     if size == "33":
-        wrong = grad_errors(got, _dqn_grads(copy.deepcopy(q).double(), d, ref_idx, rows=B - 1)[0])
+        wrong = grad_errors(got, _dqn_grads(copy.deepcopy(plain).double(), d, ref_idx, rows=B - 1)[0])
         margin = max(err / grad_bound(scale) for err, scale in wrong)
         print("  without the last row the float64 reference is %.0f x the tolerance away from the kernel" % margin)
         assert margin > 10.0
