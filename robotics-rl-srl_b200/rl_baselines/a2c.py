@@ -132,6 +132,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     last_val, adv, ret = z(H, N), z(H, T, N), z(H, T, N)
     lr_t = z(H)                              # the learning rate of each update of a replay, rewritten by the host
     params = list(policy.parameters())       # logstd (Box) first, then pi and vf: the CPU path pairs ms with them tensor by tensor
+    params0 = [p.detach().clone() for p in params]
     for p in params:
         p.grad = torch.zeros_like(p)         # static gradient tensors
     fpol = None
@@ -244,4 +245,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     env.close()
     train.best_mean_reward, train.n_saved = log.best_mean_reward, log.n_saved
     train.last_policy, train.last_norm, train.last_ms = policy, norm, ms
+    # what the last replay (or eager update) started from and left behind, for tests that rebuild it: the initial parameters, the rollout
+    # buffers of both halves, the returns and the learning rates
+    train.last_update = dict(params0=params0, buf=buf, obs=obs, adv=adv, ret=ret, last_val=last_val, lr_t=lr_t)
     return log.history

@@ -377,6 +377,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     env, on_gpu, dev, policy, dist, rank, world = run.env, run.on_gpu, run.dev, run.policy, run.dist, run.rank, run.world
     prefetch_resets, K, W = run.prefetch_resets, run.K, run.W
     params = list(policy.parameters())
+    params0 = [p.detach().clone() for p in params]
     N, T = num_envs, hp["n_steps"]
     # The GAE recursion and the minibatch step (forward, losses, backward, gradient clip, Adam) are captured into CUDA graphs too:
     # ~1000 and ~150 small launches respectively that cost more on the host than on the GPU.  Data-parallel runs keep the eager
@@ -425,17 +426,22 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
             raise ValueError("cuda_graph=True needs an even n_steps")
         side = torch.cuda.Stream(device=dev)      # library handles / workspaces are created outside the capture
         side.wait_stream(torch.cuda.current_stream(dev))
+        # the warm-up must not change what the run draws: the library's sampling counter and torch's generator (the torch policy's samples
+        # below) are restored after it, so that a captured run samples actions and minibatch permutations as an eager one does
+        rng0, torch_rng0 = fused.rng.clone() if fused is not None else None, torch.cuda.get_rng_state(dev)
         with torch.cuda.stream(side), torch.no_grad():
             for _ in range(3):
                 policy.act(obs); norm(run.e_obs if stack is None else stack, update=False)
             if fused is not None:         # first launches outside the capture (one-off function attributes); they change nothing that matters:
-                fused.act(N, obs, act_dev, buf["logp"][0], buf["val"][0], stream=env.backend.stream())     # scratch rows, one sampling counter
+                fused.act(N, obs, act_dev, buf["logp"][0], buf["val"][0], stream=env.backend.stream())
                 if K > 1:                 # a copy of the stack and a scratch output: the stack itself must not advance
                     fused.stack_filter(N, env._obs, done_u8[0], stack.clone(), torch.empty_like(obs), update=False, stream=env.backend.stream())
                 else:
                     fused.filter(N, env._obs, obs, update=False, stream=env.backend.stream())               # re-normalises the current observation
+                fused.rng.copy_(rng0)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize()
+        torch.cuda.set_rng_state(torch_rng0, dev)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):       # capture only records the launches: neither the envs nor the filter advance
             collect()
@@ -533,8 +539,10 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         else:
             gae()
         t_ph = tick("gae", t_ph)
+        perms = []
         for _ in range(hp["noptepochs"]):
             perm = torch.randperm(T * N, device=dev)
+            perms.append(perm)
             for s in range(0, T * N, mb):
                 if not graph_update:
                     zero_grads()
@@ -564,4 +572,7 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     env.close()
     train.best_mean_reward, train.n_saved = log.best_mean_reward, log.n_saved
     train.last_policy, train.last_norm = policy, norm      # for callers that want the trained objects (tests, enjoy)
+    # what the last update started from and left behind, for tests that rebuild it: the initial parameters, the rollout buffers, GAE's
+    # inputs and outputs, the epochs' permutations and the optimiser (its Adam state)
+    train.last_update = dict(params0=params0, buf=buf, obs=obs, adv=adv, ret=ret, last_val=last_val, perms=perms, opt=opt, mb=mb)
     return log.history

@@ -15,8 +15,9 @@ import numpy as np
 import pytest
 import torch
 
-from test_consumer_reference_cpu import (GAE_ULPS, filter_model, gae_model, gae_rollout, gae_torch, grad_bound, grad_errors, logp_model,
-                                         normalise, policy_model, ppo2_minibatch_grads, ppo2_policy, ppo2_rollout, CLIP, ENT_COEF, VF_COEF)
+from test_consumer_reference_cpu import (GAE_ULPS, box_sample_bound, filter_model, gae_model, gae_rollout, gae_torch, grad_bound, grad_errors,
+                                         logp_model, normalise, policy_model, ppo2_minibatch_grads, ppo2_policy, ppo2_rollout, sample_model, CLIP,
+                                         ENT_COEF, VF_COEF)
 from test_policy_cpu import _policy
 
 pytestmark = pytest.mark.gpu
@@ -167,8 +168,9 @@ def _act(lib, st, n, obs, rng, env_offset, b, first=0):
 @pytest.mark.parametrize("n", [1, 31, 32, 33, 4096, 8192])
 @pytest.mark.parametrize("discrete,obs_dim,n_out", ACT_SHAPES)
 def test_policy_act_against_a_float64_model(lib, discrete, obs_dim, n_out, n):
-    """Value and log-probability OF THE ACTION THE KERNEL DREW against the float64 towers, Box actions clipped for the env, the rollout
-    buffer copy of the observations, and the sampling counter advancing by exactly one per launch."""
+    """Value and log-probability OF THE ACTION THE KERNEL DREW against the float64 towers, the draw itself against sample_model at the launch's
+    counter, Box actions clipped for the env, the rollout buffer copy of the observations, and the sampling counter advancing by exactly one
+    per launch."""
     from srl_sim.policy import policy_struct
     pol = _policy(obs_dim, discrete, n_out, seed=40 + obs_dim * 9 + n_out).cuda()
     st, keep = policy_struct(pol)
@@ -198,8 +200,28 @@ def test_policy_act_against_a_float64_model(lib, discrete, obs_dim, n_out, n):
             z = (act - out64) / sigma
             tol = 4e-6 + 4e-7 * (np.abs(z) * (1.0 + np.abs(act)) / sigma).sum(1)
         assert (np.abs(lp - lp64) <= tol).all(), np.abs(lp - lp64).max()
+        check_draws(out64, sigma, seed, 5 + np.arange(n), launch, b["act_env"].cpu().numpy(), b["act_buf"].cpu().numpy())
         draws.append(b["act_buf"].clone())
     assert n < 8 or not torch.equal(draws[0], draws[1])                 # a new counter, new samples
+
+
+def check_draws(out64, sigma, seed, envs, counter, act_env, act_buf, label=""):
+    """The kernel's draws are sample_model's at this counter: the exact category except at draws within float32 rounding of a CDF boundary
+    (their count is printed and must stay under 0.5 % of the draws: about (n_out - 1) x 2 x 1e-5 (1 + max |logit|) of them are expected); a
+    Box sample within box_sample_bound of mean64 + sigma64 z64, and the env's action its clamp to [-1, 1].  Returns the number of near draws."""
+    want, near, z = sample_model(out64, sigma, seed, envs, counter)
+    if sigma is None:
+        bad = (act_buf != want) & ~near
+        assert not bad.any(), (label, int(bad.sum()), np.nonzero(bad)[0][:8])
+        assert near.sum() <= max(2, 5e-3 * len(want)), (label, int(near.sum()))
+        if near.any():
+            print("  %s%d of %d draws within rounding of a CDF boundary, %d of them differ" % (label, near.sum(), len(want),
+                                                                                        int((act_buf != want)[near].sum())))
+    else:
+        err = np.abs(act_buf.astype(np.float64) - want)
+        assert (err <= box_sample_bound(out64, sigma, z)).all(), (label, err.max())
+        assert np.array_equal(act_env, np.clip(act_buf, -1.0, 1.0))
+    return int(near.sum())
 
 
 def _unaligned_struct(pol):

@@ -5,7 +5,10 @@ consumer kernels (include/srl_policy.h) to these models at the trainer's shapes,
   filter_model         : VecNormalize's running moments (RunningNorm.update) as a two-pass float64 numpy merge
   normalise            : the float32 expression RunningNorm applies, on a given filter state
   policy_model         : the two 64-64 tanh towers of MlpPolicy and the log-probability of an action, in float64 numpy
+  philox_words         : Philox4x32-10 over many streams at once, in numpy
+  sample_model         : the action the policy step draws from a Philox stream, written from the distributions' definitions
   gae_torch, gae_model : the trainer's float32 torch GAE recursion, and the same recursion in float64 numpy
+  clip_adam_torch_model: nn.utils.clip_grad_norm_ followed by torch.optim.Adam (PPO2's optimiser), in float64 numpy
 """
 import copy
 
@@ -14,7 +17,7 @@ import pytest
 import torch
 
 from rl_baselines.ppo2 import RunningNorm
-from test_policy_cpu import _policy
+from test_policy_cpu import _policy, _ref_act, ref  # noqa: F401  (ref: module fixture of the CPU checker)
 
 CLIP, ENT_COEF, VF_COEF = 0.2, 0.01, 0.5           # rl_baselines.ppo2.PPO2_DEFAULTS
 
@@ -135,6 +138,68 @@ def logp_model(pol, out, act):
     return (-0.5 * z * z - ls - 0.5 * np.log(2.0 * np.pi)).sum(1)
 
 
+# ---- the policy's draws ----
+
+PURPOSE_POLICY = 16                # counter word 3 of the categorical draw; the Gaussian's block k // 4 uses 17 + k // 4
+
+
+def philox_words(seed, envs, counter, purpose):
+    """Philox4x32-10 (Salmon et al., SC'11) of the streams ``envs`` in numpy: [len(envs), 4] uint32 words.  Key = seed; counter = (env lo,
+    env hi, ``counter``, ``purpose``)."""
+    M = np.uint64(0xFFFFFFFF)
+    env = np.asarray(envs, np.uint64).reshape(-1)
+    c0, c1 = env & M, env >> np.uint64(32)
+    c2, c3 = np.full_like(c0, int(counter) & 0xFFFFFFFF), np.full_like(c0, int(purpose) & 0xFFFFFFFF)
+    k0, k1 = int(seed) & 0xFFFFFFFF, (int(seed) >> 32) & 0xFFFFFFFF
+    for _ in range(10):
+        p0, p1 = c0 * np.uint64(0xD2511F53), c2 * np.uint64(0xCD9E8D57)        # 32 x 32 -> 64 bits: no wrap in uint64
+        c0, c1, c2, c3 = (p1 >> np.uint64(32)) ^ c1 ^ np.uint64(k0), p1 & M, (p0 >> np.uint64(32)) ^ c3 ^ np.uint64(k1), p0 & M
+        k0, k1 = (k0 + 0x9E3779B9) & 0xFFFFFFFF, (k1 + 0xBB67AE85) & 0xFFFFFFFF
+    return np.stack([c0, c1, c2, c3], 1).astype(np.uint32)
+
+
+def u53(words):
+    """The 53-bit uniform in [0, 1) of words 0 and 1 (numpy's random_sample construction)."""
+    w = words.astype(np.float64)
+    return (np.floor(w[:, 0] / 32.0) * 67108864.0 + np.floor(w[:, 1] / 64.0)) / 9007199254740992.0
+
+
+def sample_model(out64, sigma, seed, envs, counter, near_tol=None):
+    """The action drawn for each env of ``envs`` at sampling counter ``counter``, in float64 from the distributions' definitions.
+    ``out64`` [n, n_out]: logits (``sigma`` None) or Gaussian means (``sigma`` [n_out]: the standard deviations).
+      Categorical: inverse CDF of softmax(logits) at u = the 53-bit uniform of words 0 and 1 of Philox (seed; env; counter; 16).
+      Gaussian:    Box-Muller on 24-bit uniforms (w >> 8 + 1/2) / 2^24.  Dimension k takes block 17 + k // 4; words (0, 1) are the pair of
+                   k % 4 = 0 (cos) and 1 (sin), words (2, 3) the pair of k % 4 = 2 (cos) and 3 (sin).
+    Returns (action, near, z): ``near`` marks categorical draws whose u lies within ``near_tol`` (per row; default 1e-5 (1 + max |logit|),
+    the float32 rounding of logits, exponentials and the running CDF sum) of a CDF boundary, where a float32 computation may take either
+    side; ``z`` [n, n_out] are the Gaussian's standard normals (None for a categorical)."""
+    out64 = np.asarray(out64, np.float64)
+    n, A = out64.shape
+    if sigma is None:
+        u = u53(philox_words(seed, envs, counter, PURPOSE_POLICY))
+        p = np.exp(out64 - out64.max(1, keepdims=True))
+        cdf = np.cumsum(p / p.sum(1, keepdims=True), 1)[:, :-1]               # the last boundary is 1: u < 1 always
+        act = (cdf <= u[:, None]).sum(1)
+        tol = 1e-5 * (1.0 + np.abs(out64).max(1)) if near_tol is None else near_tol
+        near = (np.abs(cdf - u[:, None]) <= np.reshape(tol, (-1, 1))).any(1) if A > 1 else np.zeros(n, bool)
+        return act, near, None
+    z = np.zeros((n, A))
+    for k in range(A):
+        w = philox_words(seed, envs, counter, PURPOSE_POLICY + 1 + k // 4).astype(np.float64)
+        j = k & 2
+        u1, u2 = (np.floor(w[:, j] / 256.0) + 0.5) / 16777216.0, (np.floor(w[:, j + 1] / 256.0) + 0.5) / 16777216.0
+        rad, ang = np.sqrt(-2.0 * np.log(u1)), 2.0 * np.pi * u2
+        z[:, k] = rad * (np.sin(ang) if k & 1 else np.cos(ang))
+    return out64 + np.asarray(sigma, np.float64) * z, np.zeros(n, bool), z
+
+
+def box_sample_bound(out64, sigma, z):
+    """How far a float32 draw may sit from mean64 + sigma64 z64: the float32 towers' error on the mean (the value tolerance of the kernel
+    tests, 2e-5 + 1e-6 |mean|), float32 logf / sqrtf / sinf / cosf on z (a few ulps: 1e-6 (1 + |z|) with margin) scaled by sigma, and the
+    rounding of the final fused multiply-add."""
+    return 2e-5 + 2e-6 * np.abs(out64) + 2e-6 * np.asarray(sigma) * (1.0 + np.abs(z))
+
+
 # ---- GAE ----
 
 def gae_torch(rew, val, done, last_val, gamma, lam):
@@ -180,6 +245,41 @@ def gae_rollout(T, N, device, seed):
 
 
 GAE_ULPS = 8       # float32 recursion vs float64, in float32 ulps (2^-23) of the tensor's largest magnitude: up to 3.3 at T = 129
+
+
+# ---- PPO2's optimiser ----
+
+def clip_grad_norm_model(grads, max_norm):
+    """nn.utils.clip_grad_norm_: the global 2-norm over every tensor, coef = max_norm / (norm + 1e-6) clamped at 1.  Returns (clipped grads, coef)."""
+    norm = np.sqrt(sum(float((np.asarray(g, np.float64) ** 2).sum()) for g in grads))
+    coef = min(1.0, max_norm / (norm + 1e-6))
+    return [np.asarray(g, np.float64) * coef for g in grads], coef
+
+
+def adam_torch_model(params, grads, m, v, step, lr, beta1=0.9, beta2=0.999, eps=1e-5):
+    """Step ``step`` (1-based) of torch.optim.Adam without weight decay or amsgrad: bias-corrected moments, eps added AFTER the square root
+    (torch's formula; TF's Adam in tests/deepq_numpy_ref.py adds it to the uncorrected root).  Returns (params, m, v)."""
+    bc1, bc2 = 1.0 - beta1 ** step, 1.0 - beta2 ** step
+    new_p, new_m, new_v = [], [], []
+    for p, g, mk, vk in zip(params, grads, m, v):
+        mk = beta1 * np.asarray(mk, np.float64) + (1.0 - beta1) * g
+        vk = beta2 * np.asarray(vk, np.float64) + (1.0 - beta2) * g * g
+        new_p.append(np.asarray(p, np.float64) - (lr / bc1) * mk / (np.sqrt(vk) / np.sqrt(bc2) + eps))
+        new_m.append(mk)
+        new_v.append(vk)
+    return new_p, new_m, new_v
+
+
+def clip_adam_torch_model(params, grad_steps, lr, max_norm=0.5, eps=1e-5):
+    """PPO2's optimiser over a sequence of raw gradients (lists of arrays), from zero Adam slots: clip_grad_norm_(max_norm) then one Adam step
+    each.  Returns (params, m, v, clipped gradients of every step)."""
+    p = [np.asarray(x, np.float64) for x in params]
+    m, v, clipped = [np.zeros_like(x) for x in p], [np.zeros_like(x) for x in p], []
+    for s, g in enumerate(grad_steps):
+        gc, _ = clip_grad_norm_model(g, max_norm)
+        clipped.append(gc)
+        p, m, v = adam_torch_model(p, gc, m, v, s + 1, lr, eps=eps)
+    return p, m, v, clipped
 
 
 # ---- CPU checks of the references ----
@@ -261,3 +361,93 @@ def test_gae_references_agree(T, N):
             assert np.abs(got.numpy() - want).max() <= GAE_ULPS * 2.0 ** -23 * np.abs(want).max()
         if T == 1:      # no recursion: adv = rew + gamma * last_val * (1 - done) - val
             assert np.allclose(a64[0], (rew[0] + gamma * last_val * (1 - done[0]) - val[0]).numpy(), rtol=1e-6, atol=1e-6)
+
+
+def test_numpy_philox_matches_the_oracle(oracle_lib):
+    """philox_words equals the oracle's Philox4x32-10 (itself held to the published known-answer vectors in tests/test_mobile_cpu.py) word for
+    word, over streams that cross 2^32, counters up to 2^32 - 1, every policy purpose and a 64-bit key."""
+    import ctypes
+    fn = oracle_lib.lib.oracle_philox4x32
+    fn.argtypes = [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32)]
+    fn.restype = None
+    out = (ctypes.c_uint32 * 4)()
+    envs = [0, 1, 7, 4095, 4096, 2 ** 32 - 1, 2 ** 32 + 5, 2 ** 63 + 3]
+    for seed in (0, 1234, 0x299F31D0A4093822):
+        for counter in (0, 1, 31, 2 ** 32 - 1):
+            for purpose in (16, 17, 18):
+                got = philox_words(seed, envs, counter, purpose)
+                for i, e in enumerate(envs):
+                    fn(seed, e, counter, purpose, out)
+                    assert list(got[i]) == list(out), (seed, e, counter, purpose)
+    w = np.array([[0, 0, 0, 0], [0xFFFFFFFF, 0xFFFFFFFF, 0, 0], [0x80000000, 0, 0, 0]], np.uint32)
+    assert list(u53(w)) == [0.0, 1.0 - 2.0 ** -53, 0.5]
+
+
+@pytest.mark.parametrize("discrete,obs_dim,n_out", [(True, 3, 1), (True, 3, 3), (True, 12, 7), (False, 3, 1), (False, 3, 3), (False, 12, 7)])
+def test_sample_model_matches_the_checker_draws(ref, discrete, obs_dim, n_out):
+    """The host checker (csrc/policy_core.h compiled for the CPU) draws what sample_model says, at the float64 towers' outputs: the same category
+    except at the few draws within rounding of a CDF boundary, and Gaussian samples within float32 of mean64 + sigma64 z64.  n_out = 7 is the
+    Gaussian's two-block case.  Two counters and an env offset check the stream each draw takes; the models of two natural mistakes (every
+    Gaussian dimension from the first word pair, a CDF from half the logits) are far from the checker."""
+    pol = _policy(obs_dim, discrete, n_out, seed=60 + obs_dim + n_out)
+    n = 6000
+    obs = torch.randn(n, obs_dim, generator=torch.Generator().manual_seed(obs_dim)) * 1.5
+    out64, _ = policy_model(pol, obs.numpy())
+    sigma = None if discrete else np.exp(pol.logstd.detach().double().numpy())
+    for seed, counter, off in ((5, 0, 0), (1234, 3, 4096)):
+        _, act_buf, _, _, _ = _ref_act(ref, pol, obs, seed=seed, counter=counter, env_offset=off)
+        act, near, z = sample_model(out64, sigma, seed, np.arange(n) + off, counter)
+        if discrete:
+            same = act_buf == act
+            print("\n%s n_out=%d counter %d: %d of %d draws near a CDF boundary, %d of them differ" % (discrete, n_out, counter, near.sum(), n,
+                                                                                                     (~same[near]).sum()))
+            assert same[~near].all(), np.nonzero(~same & ~near)[0][:10]
+            assert near.sum() <= 2e-3 * n
+            if n_out > 1:
+                assert len(np.unique(act)) == n_out
+                p = np.exp(0.5 * (out64 - out64.max(1, keepdims=True)))
+                u = u53(philox_words(seed, np.arange(n) + off, counter, PURPOSE_POLICY))
+                half = (np.cumsum(p / p.sum(1, keepdims=True), 1)[:, :-1] <= u[:, None]).sum(1)
+                assert (half != act_buf).mean() > 0.01
+        else:
+            err = np.abs(act_buf - act)
+            assert (err <= box_sample_bound(out64, sigma, z)).all(), err.max()
+            assert 0.9 < z.std() < 1.1 and abs(z.mean()) < 0.1
+            if n_out > 2:                               # dims 2 and 3 from words (2, 3), not again from words (0, 1)
+                assert np.abs(act_buf[:, 2] - (out64[:, 2] + sigma[2] * z[:, 0])).max() > 0.1
+            if n_out > 4:                               # dim 4 from a second block, not again from the first
+                assert np.abs(act_buf[:, 4] - (out64[:, 4] + sigma[4] * z[:, 0])).max() > 0.1
+
+
+def test_clip_adam_model_matches_torch():
+    """clip_adam_torch_model is nn.utils.clip_grad_norm_(0.5) + torch.optim.Adam(eps=1e-5) in float64 over four steps: one gradient far above the
+    clip norm, one below it, one at about twice it, one of zeros (the moments decay, the step stays finite).  torch runs the CPU Adam
+    implementation here; the trainer's capturable CUDA Adam states the same formula."""
+    g = torch.Generator().manual_seed(3)
+    shapes = [(64, 3), (64,), (64, 64), (6,)]
+    params = [torch.randn(s, generator=g, dtype=torch.float64, requires_grad=True) for s in shapes]
+    p0 = [p.detach().numpy().copy() for p in params]
+    opt = torch.optim.Adam(params, lr=2.5e-4, eps=1e-5)
+    steps = []
+    for scale in (3.0, 0.001, 0.01, 0.0):
+        grads = [torch.randn(s, generator=g, dtype=torch.float64) * scale for s in shapes]
+        steps.append([x.numpy().copy() for x in grads])
+        for p, x in zip(params, grads):
+            p.grad = x.clone()
+        torch.nn.utils.clip_grad_norm_(params, 0.5)
+        opt.step()
+    assert np.sqrt(sum((x ** 2).sum() for x in steps[0])) > 10 * 0.5 and np.sqrt(sum((x ** 2).sum() for x in steps[1])) < 0.5
+    got_p, got_m, got_v, clipped = clip_adam_torch_model(p0, steps, 2.5e-4)
+    for k, p in enumerate(params):
+        st = opt.state[p]
+        assert float(st["step"]) == 4.0
+        assert np.allclose(got_m[k], st["exp_avg"].numpy(), rtol=1e-12, atol=1e-300)
+        assert np.allclose(got_v[k], st["exp_avg_sq"].numpy(), rtol=1e-12, atol=1e-300)
+        assert np.allclose(got_p[k], p.detach().numpy(), rtol=0, atol=1e-15)
+    assert np.allclose(np.sqrt(sum((x ** 2).sum() for x in clipped[0])), 0.5 / (1.0 + 1e-6 / np.sqrt(sum((x ** 2).sum() for x in steps[0]))), rtol=1e-12)
+    assert all(np.array_equal(a, b) for a, b in zip(clipped[1], steps[1]))
+    # TF's Adam (eps on the uncorrected root) differs visibly after one step at this eps: the model is torch's, not TF's
+    _, m1, v1 = adam_torch_model(p0, clipped[1], [np.zeros_like(x) for x in p0], [np.zeros_like(x) for x in p0], 1, 1.0)
+    tf_move = np.sqrt(1 - 0.999) / (1 - 0.9) * m1[1] / (np.sqrt(v1[1]) + 1e-5)
+    torch_move = m1[1] / (1 - 0.9) / (np.sqrt(v1[1]) / np.sqrt(1 - 0.999) + 1e-5)
+    assert np.abs(tf_move - torch_move).max() > 1e-3

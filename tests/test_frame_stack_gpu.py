@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_consumer_kernels_gpu import CH, _act, _act_buffers, _grad_mb, _sms, _stream, lib  # noqa: F401  (lib: module fixture)
+from test_consumer_kernels_gpu import CH, _act, _act_buffers, _grad_mb, _sms, _stream, check_draws, lib  # noqa: F401  (lib: module fixture)
 from test_consumer_reference_cpu import (filter_model, grad_bound, grad_errors, logp_model, normalise, policy_model, ppo2_minibatch_grads, ppo2_policy,
                                          ppo2_rollout, CLIP, ENT_COEF, VF_COEF)
 from test_policy_cpu import _policy, _ref_act, ref  # noqa: F401  (ref: module fixture of the CPU checker)
@@ -94,8 +94,9 @@ WIDE_HEADS = [(True, 6), (False, 3), (False, 7)]
 @pytest.mark.parametrize("discrete,n_out", WIDE_HEADS)
 @pytest.mark.parametrize("obs_dim", WIDE)
 def test_wide_policy_act_against_float64_and_the_checker(lib, ref, obs_dim, discrete, n_out, n):  # noqa: F811
-    """Value and log-probability of the drawn action against the float64 towers (the tolerances of test_consumer_kernels_gpu.py), the rollout
-    copy of the observations, the counter; the samples against the CPU checker's (an ulp of expf / tanhf may move a CDF boundary)."""
+    """Value and log-probability of the drawn action against the float64 towers (the tolerances of test_consumer_kernels_gpu.py), the draws
+    against sample_model, the rollout copy of the observations, the counter; the samples against the CPU checker's (an ulp of expf / tanhf may
+    move a CDF boundary)."""
     from srl_sim.policy import policy_struct
     pol = _policy(obs_dim, discrete, n_out, seed=500 + obs_dim * 9 + n_out).cuda()
     st, keep = policy_struct(pol)
@@ -126,6 +127,7 @@ def test_wide_policy_act_against_float64_and_the_checker(lib, ref, obs_dim, disc
         z = (act - out64) / sigma
         tol = 4e-6 + 4e-7 * (np.abs(z) * (1.0 + np.abs(act)) / sigma).sum(1)
     assert (np.abs(lp - lp64) <= tol).all(), np.abs(lp - lp64).max()
+    check_draws(out64, sigma, seed, 3 + np.arange(n), 0, b["act_env"].cpu().numpy(), b["act_buf"].cpu().numpy())
 
 
 # ---------------------------------------------------------------- srl_ppo2_grad, wide
