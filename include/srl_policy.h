@@ -19,6 +19,10 @@
  *                   <- stable-baselines 2.5 `DQN.learn` with the deepq `MlpPolicy` (chosen by rl_baselines/rl_algorithm/deepq.py): the
  *                      epsilon-greedy `act`, baselines' `PrioritizedReplayBuffer` (add, sample, update_priorities) and `build_train`'s double-Q
  *                      loss, `tf.clip_by_norm` per gradient tensor and `tf.train.AdamOptimizer`
+ *   srl_sac_act, srl_sac_store, srl_sac_prepare, srl_sac_grad, srl_sac_adam
+ *                   <- stable-baselines 2.5 `SAC.learn` with its `MlpPolicy` (chosen by rl_baselines/rl_algorithm/sac.py): the policy step,
+ *                      `ReplayBuffer.add` / `sample`, the losses and `tf.gradients` of `SAC.setup_model`, its three `tf.train.AdamOptimizer`s
+ *                      and the Polyak target update
  *
  * Conventions are those of srl_sim.h: 0 on success, message from srl_sim_last_error(); all pointers are DEVICE pointers;
  * calls are asynchronous on `stream` and capturable into a CUDA graph (everything a launch reads that changes between
@@ -209,6 +213,80 @@ int srl_replay_sample(const srl_replay_tree* t, int batch, int prioritized, cons
  * priority of its LAST occurrence in the batch), max_priority = max(max_priority, p), then every internal node is rebuilt bottom-up.
  * idx entries must be stored transitions (0 <= idx < size). */
 int srl_replay_update(const srl_replay_tree* t, int batch, const int64_t* idx, const float* td, double alpha, float eps, void* stream);
+
+/* ---- SAC (rl_baselines/sac.py) ----
+ * stable-baselines 2.5 `SAC` with its `MlpPolicy` (chosen by rl_baselines/rl_algorithm/sac.py).  Five 64-64 ReLU networks, each
+ * in -> 64 -> 64 -> out in torch.nn.Linear layout (w1 [64][in], b1 [64], w2 [64][64], b2 [64], w3 [out][64], b3 [out]):
+ *   actor     W -> 2A: rows 0..A-1 of w3 / b3 are the `mu` head, rows A..2A-1 the `log_std` head, log_std = clip(., -20, 2)
+ *   qf1, qf2  W + A -> 1 on concat(obs, action), obs first
+ *   vf        W -> 1;  the target vf has vf's layout in a separate array
+ * W = obs_dim 1..32, A = act_dim 1..8.  The parameters live in one flat f32 ARENA in the order actor | qf1 | qf2 | vf | log_ent_coef (one
+ * float), each network's six tensors in the order above; srl_sac_arena_floats gives its length P.  The gradient and the Adam slots m, v are
+ * arrays of the same layout.
+ * RECALLED from stable-baselines 2.5, not checked against an installed copy (none can be installed here): the networks and their init, the
+ * log_std clip and its gradient (zero strictly outside [-20, 2], passed at the bounds), the log-probability as the TF graph writes it, the
+ * losses and which optimiser owns which variables, TF1 Adam, the Polyak update after the Adam steps, and the learn loop's conditions.
+ * Philox purposes (counter word 3; DQN uses 24 and 25): 26, 27 the acting noise of dims 0-3 / 4-7; 28, 29 the uniform random action of
+ * dims 0-3 / 4-7; 30 the sample index; 31, 32 the reparameterisation noise of dims 0-3 / 4-7 of a sample.  Gaussian words are those of
+ * srl_sample_gaussian (Box-Muller on 24-bit uniforms, dims 4j..4j+3 from one block: cos / sin of words (0, 1), then of words (2, 3)).
+ * Every entry point is asynchronous on `stream`, capturable (counters, step, learning rate and log_ent_coef live in device memory) and
+ * deterministic (fixed-order reductions). */
+typedef struct srl_sac_nets {
+    uint32_t struct_size;   /* = sizeof(srl_sac_nets); checked            */
+    int32_t  obs_dim;       /* W, 1..32                                    */
+    int32_t  act_dim;       /* A, 1..8                                     */
+    int32_t  reserved;
+    float*   arena;         /* f32[P]: actor | qf1 | qf2 | vf | log_ent_coef */
+    float*   target;        /* f32[vf's size]: the target value network    */
+} srl_sac_nets;
+
+size_t srl_sac_arena_floats(int obs_dim, int act_dim);   /* P; 0 for an unsupported shape */
+
+/* The action of n envs from the observations obs (f32[n, obs_dim]).  mode 0: sample, a = tanh(mu + std z) with std = exp(clip(log_std)),
+ * z_k Gaussian from the Philox stream (seed, env_offset + i, counter) with purposes 26 + k / 4;  mode 1: deterministic, a = tanh(mu);
+ * mode 2: uniform random, a_k = 2 (word >> 8) / 2^24 - 1 from word k % 4 of purpose 28 + k / 4 (the network is not evaluated).
+ *   rng : u64[3] {seed, counter, 0}; the launch advances the counter by one when its last CTA retires (srl_policy_act's rule)
+ *   act_out : f32[n, act_dim], the squashed action for srl_sim_step and the replay ring */
+int srl_sac_act(const srl_sac_nets* nets, int n, const float* obs, int mode, uint64_t* rng, uint64_t env_offset, float* act_out, void* stream);
+
+/* The replay ring of `rows` rows of n transitions: row r = (*step) % rows receives obs, act, rew, done and new_obs (ring arrays obs_ring,
+ * next_obs_ring f32[rows, n, obs_dim], act_ring f32[rows, n, act_dim], rew_ring f32[rows, n], done_ring u8[rows, n]); then obs <- new_obs
+ * in place (the next step's observation) and step[0] += 1.  step : i64[2] {lockstep steps stored, 0} (word 1 counts the launch's retired
+ * CTAs).  The row comes from device memory, so one captured launch serves every row. */
+int srl_sac_store(int rows, int n, int obs_dim, int act_dim, int64_t* step, float* obs, const float* act, const float* rew, const uint8_t* done,
+                  const float* new_obs, float* obs_ring, float* act_ring, float* rew_ring, uint8_t* done_ring, float* next_obs_ring, void* stream);
+
+/* The per-sample part of one gradient step over `batch` samples drawn from the size = min(*step, rows) * n stored transitions:
+ *   sample b: u a 53-bit uniform of words 0-1 of the stream (seed, b, counter), purpose 30; g = min(floor(u size), size - 1) -> idx[b]
+ *   q_backup[b] = rew[g] + gamma ((1 - done[g]) V_targ(next_obs[g]))
+ *   actor at obs[g]: mu, ls = clip(log_std, -20, 2), eps_k Gaussian (stream (seed, b, counter), purposes 31 + k / 4), u = mu + exp(ls) eps,
+ *     a_pi = tanh(u), logp[b] = sum_k -0.5 (((u - mu) / (exp(ls) + 1e-6))^2 + 2 ls + log 2 pi) - sum_k log(1 - a_pi^2 + 1e-6)
+ *   v_backup[b] = min(qf1(obs, a_pi), qf2(obs, a_pi)) - alpha logp[b],  alpha = exp(log_ent_coef) (auto_ent) or ent_coef
+ *   d_actor[b] : f32[batch, 2 act_dim], d policy_loss / d (mu, raw log_std) of the sample, policy_loss = mean(alpha logp - qf1(obs, a_pi)),
+ *                through qf1's input gradient; the log_std part is 0 where the raw head is outside [-20, 2]
+ *   ent_grad : f32[1], d ent_coef_loss / d log_ent_coef = -mean(logp + target_entropy), summed in float64 in a fixed order (0 unless auto_ent);
+ *              it may point at log_ent_coef's entry of the gradient arena.  rng as for srl_sac_act (its own record).
+ * With nothing stored (step[0] == 0) every idx[b] is -1 and every output is 0; srl_sac_grad then writes a zero gradient. */
+int srl_sac_prepare(const srl_sac_nets* nets, int rows, int n, const int64_t* step, const float* obs_ring, const float* act_ring, const float* rew_ring,
+                    const uint8_t* done_ring, const float* next_obs_ring, int batch, float gamma, int auto_ent, float ent_coef, float target_entropy,
+                    uint64_t* rng, int64_t* idx, float* q_backup, float* v_backup, float* logp, float* d_actor, float* ent_grad, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
+/* The weight gradients of one step, written into `grad` (f32[P], every entry but log_ent_coef's, which srl_sac_prepare writes):
+ *   actor from d_actor;  qf_i from qf_i_loss = 0.5 mean((q_backup - qf_i(obs, act))^2) at the STORED action;  vf from
+ *   value_loss = 0.5 mean((vf(obs) - v_backup)^2).  Each network's forward pass is recomputed in chunks of 64 samples with every activation
+ *   in shared memory; per-CTA partial gradients are summed in float64 in CTA order.  idx, q_backup, v_backup, d_actor as srl_sac_prepare left them.
+ *   workspace : at least srl_sac_workspace_bytes(obs_dim, act_dim, batch) bytes (shared with srl_sac_prepare; no state between calls) */
+size_t srl_sac_workspace_bytes(int obs_dim, int act_dim, int batch);
+int srl_sac_grad(const srl_sac_nets* nets, int n, const float* obs_ring, const float* act_ring, int batch, const int64_t* idx, const float* q_backup,
+                 const float* v_backup, const float* d_actor, float* grad, void* workspace, size_t workspace_bytes, void* stream);
+
+/* TF1 Adam over the whole arena in srl_clip_adam's statement and order of roundings (no clipping), then, when `polyak`, the target update
+ * target = (1 - tau) target + tau vf from the updated vf, in float32:  m += (g - m)(1 - beta1); v += (g^2 - v)(1 - beta2);
+ * lr_t = lr sqrt(1 - beta2^t) / (1 - beta1^t); w -= m lr_t / (sqrt(v) + epsilon).  One launch; the three optimisers of stable-baselines'
+ * SAC step together, so one beta_power f32[2] {beta1^t, beta2^t} serves them all (multiplied by {beta1, beta2} after the step).  lr : f32[1]. */
+int srl_sac_adam(const srl_sac_nets* nets, const float* grad, float* m, float* v, const float* lr, float* beta_power, float beta1, float beta2,
+                 float epsilon, int polyak, float tau, void* stream);
 
 #ifdef __cplusplus
 }

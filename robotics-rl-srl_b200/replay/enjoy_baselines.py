@@ -2,7 +2,8 @@
 Mirror of the reference's replay entry point ``python -m replay.enjoy_baselines --log-dir <trained agent>``
 (replay/enjoy_baselines.py:45-63 arguments, :66-118 config loading, :151-333 the enjoy loop) for the agents this repo can
 train: it reloads ``args.json`` / ``env_globals.json`` / ``<algo>_model.pt`` written by ``rl_baselines.ppo2.train`` or ``rl_baselines.a2c.train``
-(the same MlpPolicy) or ``rl_baselines.deepq.train`` (the dueling Q network, always greedy: stable-baselines' DQN.predict), rebuilds the
+(the same MlpPolicy), ``rl_baselines.deepq.train`` (the dueling Q network, always greedy: stable-baselines' DQN.predict) or ``rl_baselines.sac.train``
+(the squashed Gaussian actor: ``tanh(mu)`` with ``--deterministic``, a sample otherwise), rebuilds the
 env batch with the training-time keyword arguments and the saved observation filter (``load_path_normalise``, :145), runs the
 policy for ``--num-timesteps`` steps and reports ``"<n> episodes - Mean reward: <r>"`` like the reference (:330-333).
 Rendering / plotting flags are accepted and ignored (image observations are out of scope, DESIGN.md section 8).
@@ -41,7 +42,7 @@ def loadConfigAndSetup(load_args):
     with open(os.path.join(log_dir, "args.json")) as f:
         train_args = json.load(f)
     algo = train_args.get("algo", "ppo2")
-    if algo not in ("ppo2", "a2c", "deepq"):
+    if algo not in ("ppo2", "a2c", "deepq", "sac"):
         raise ValueError(algo + " is not supported for replay")
     env_kwargs = dict(env_globals)
     env_kwargs["shape_reward"] = load_args.shape_reward            # reward sparse or shaped: chosen at replay time (:88)
@@ -60,8 +61,11 @@ def main(argv=None):
     D = env.observation_space.shape[0]
     K = int(train_args.get("num_stack", 1))                       # VecFrameStack of the training run (:140)
     W = K * D
-    deepq = train_args.get("algo") == "deepq"
-    if deepq:
+    deepq, sac = train_args.get("algo") == "deepq", train_args.get("algo") == "sac"
+    if sac:
+        from rl_baselines.sac import SACNets
+        policy = SACNets(W, env.action_space.shape[0]).to(dev)
+    elif deepq:
         from rl_baselines.deepq import DuelingQ
         policy = DuelingQ(W, env.action_space.n).to(dev)
     else:
@@ -80,7 +84,9 @@ def main(argv=None):
     n_done, returns = 0, []
     with torch.no_grad():
         for _ in range(load_args.num_timesteps):
-            if deepq:
+            if sac:
+                a = policy.act(obs, deterministic=load_args.deterministic)
+            elif deepq:
                 a = policy(obs).argmax(-1)
             else:
                 dist = policy.dist(obs)

@@ -1,7 +1,7 @@
 """
 Mirror of the reference's training entry point ``python -m rl_baselines.train`` (rl_baselines/train.py:172-333) for the
 algorithms this repo provides as consumers of the simulator: ``ppo2`` (rl_baselines/ppo2.py), ``a2c`` (rl_baselines/a2c.py), ``deepq``
-(rl_baselines/deepq.py) and ``random_agent`` (rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the
+(rl_baselines/deepq.py), ``sac`` (rl_baselines/sac.py) and ``random_agent`` (rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the
 batch (per GPU when launched with ``torchrun --nproc-per-node N -m rl_baselines.train``: data-parallel PPO2, A2C or DQN, see rl_baselines/ppo2.py).
 """
 import argparse
@@ -19,7 +19,9 @@ A2C_OPT_PARAM = {"n_steps": int, "vf_coef": float, "ent_coef": float, "max_grad_
 # rl_baselines/rl_algorithm/deepq.py:65-75 (DQNModel.getOptParam)
 DQN_OPT_PARAM = {"learning_rate": float, "exploration_fraction": float, "exploration_final_eps": float, "train_freq": int, "learning_starts": int,
                  "target_network_update_freq": int, "gamma": float, "batch_size": int}
-OPT_PARAM = {"ppo2": PPO2_OPT_PARAM, "a2c": A2C_OPT_PARAM, "deepq": DQN_OPT_PARAM}
+# rl_baselines/rl_algorithm/sac.py (SACModel.getOptParam)
+SAC_OPT_PARAM = {"ent_coef": float, "learning_rate": float, "gradient_steps": int, "train_freq": int}
+OPT_PARAM = {"ppo2": PPO2_OPT_PARAM, "a2c": A2C_OPT_PARAM, "deepq": DQN_OPT_PARAM, "sac": SAC_OPT_PARAM}
 LR_SCHEDULES = ['linear', 'constant', 'double_linear_con', 'middle_drop', 'double_middle_drop']
 
 
@@ -38,13 +40,13 @@ def parserHyperParam(pairs, opt_param=PPO2_OPT_PARAM):
 
 def main(argv=None):
     parser = argparse.ArgumentParser(description="Train script for RL algorithms")
-    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'a2c', 'deepq', 'random_agent'], type=str)
+    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'a2c', 'deepq', 'sac', 'random_agent'], type=str)
     parser.add_argument('--env', type=str, help='environment ID', default='KukaButtonGymEnv-v0', choices=list(registered_env.keys()))
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--episode_window', type=int, default=40, help='Episode window for moving average plot (default: 40)')
     parser.add_argument('--num-stack', type=int, default=1, help='number of frames to stack (default: 1)')
     parser.add_argument('-joints', '--action-joints', action='store_true', default=False, help='set actions to the joints of the arm directly')
-    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 / A2C / DQN hyper-parameters as name:value pairs')
+    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 / A2C / DQN / SAC hyper-parameters as name:value pairs')
     parser.add_argument('--lr-schedule', help='Learning rate schedule (a2c)', default='constant', choices=LR_SCHEDULES)
     parser.add_argument('--log-dir', default='/tmp/gym/', type=str)
     parser.add_argument('--num-timesteps', type=int, default=int(1e6))
@@ -58,7 +60,7 @@ def main(argv=None):
     # deepq's own flags (rl_algorithm/deepq.py:20-24); --dueling is accepted and has no effect: the deepq MlpPolicy is dueling either way
     parser.add_argument('--prioritized', type=int, default=1)
     parser.add_argument('--dueling', type=int, default=1)
-    parser.add_argument('--buffer-size', type=int, default=int(1e3), help="Replay buffer size")
+    parser.add_argument('--buffer-size', type=int, default=None, help="Replay buffer size (default: 1000 for deepq, 50000 for sac)")
     args, _ = parser.parse_known_args(argv)
     # sanity checks of the reference (train.py:221-224,265-266)
     assert args.episode_window >= 1, "Error: --episode_window cannot be less than 1"
@@ -70,22 +72,29 @@ def main(argv=None):
     if args.algo == "deepq" and args.continuous_actions:       # train.py:260-262
         from rl_baselines.deepq import CONTINUOUS_ERROR
         raise ValueError(CONTINUOUS_ERROR)
+    if args.algo == "sac" and not args.continuous_actions:    # train.py:257-259
+        from rl_baselines.sac import DISCRETE_ERROR
+        raise ValueError(DISCRETE_ERROR)
     hyperparams = parserHyperParam(args.hyperparam, OPT_PARAM.get(args.algo, PPO2_OPT_PARAM))
     if args.algo == "a2c":
         hyperparams = dict(dict(lr_schedule=args.lr_schedule), **hyperparams)
     if args.algo == "deepq":
-        hyperparams = dict(dict(buffer_size=args.buffer_size, prioritized_replay=bool(args.prioritized)), **hyperparams)
+        hyperparams = dict(dict(buffer_size=args.buffer_size or int(1e3), prioritized_replay=bool(args.prioritized)), **hyperparams)
+    if args.algo == "sac":
+        hyperparams = dict(dict(buffer_size=args.buffer_size or 50000), **hyperparams)
     env_kwargs = dict(is_discrete=not args.continuous_actions, action_repeat=args.action_repeat, random_target=args.random_target,
                       shape_reward=args.shape_reward, srl_model=args.srl_model)
     if args.action_joints:
         env_kwargs["action_joints"] = True
     log_dir = os.path.join(args.log_dir, args.env, args.srl_model, args.algo, time.strftime("%y-%m-%d_%Hh%M_%S"))
     num_timesteps = int(1.1 * args.num_timesteps)      # the reference trains 10 % longer (train.py:319)
-    if args.algo in ("ppo2", "a2c", "deepq"):
+    if args.algo in ("ppo2", "a2c", "deepq", "sac"):
         if args.algo == "ppo2":
             from rl_baselines.ppo2 import train
         elif args.algo == "a2c":
             from rl_baselines.a2c import train
+        elif args.algo == "sac":
+            from rl_baselines.sac import train
         else:
             from rl_baselines.deepq import train
         from srl_sim.distributed import rank_world

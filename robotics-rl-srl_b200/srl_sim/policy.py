@@ -14,7 +14,8 @@ from ctypes import POINTER, Structure, byref, c_double, c_float, c_int, c_int32,
 HIDDEN, MAX_OBS, MAX_OUT = 64, 32, 8     # observation widths 1..8 and 9..32 (stacked states) run separate kernel instantiations
 POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "srl_ppo2_grad", "srl_ppo2_workspace_bytes", "srl_ppo2_gae",
                   "srl_a2c_grad", "srl_a2c_workspace_bytes", "srl_clip_rmsprop", "srl_dqn_act", "srl_dqn_target", "srl_dqn_grad", "srl_clip_adam",
-                  "srl_replay_add", "srl_replay_sample", "srl_replay_update"]
+                  "srl_replay_add", "srl_replay_sample", "srl_replay_update", "srl_sac_arena_floats", "srl_sac_workspace_bytes", "srl_sac_act",
+                  "srl_sac_store", "srl_sac_prepare", "srl_sac_grad", "srl_sac_adam"]
 GRAD_NAMES = ["pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3", "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3", "logstd"]
 
 
@@ -36,6 +37,11 @@ class SrlReplayTree(Structure):
     """struct srl_replay_tree (include/srl_policy.h)."""
     _fields_ = [("struct_size", c_uint32), ("n_envs", c_int32), ("capacity", c_int64), ("tree_cap", c_int64)] + \
                [(name, c_void_p) for name in ("sum", "min", "max_priority", "size", "stamp")]
+
+
+class SrlSacNets(Structure):
+    """struct srl_sac_nets (include/srl_policy.h)."""
+    _fields_ = [("struct_size", c_uint32), ("obs_dim", c_int32), ("act_dim", c_int32), ("reserved", c_int32), ("arena", c_void_p), ("target", c_void_p)]
 
 
 def bind(cdll):
@@ -77,6 +83,22 @@ def bind(cdll):
     cdll.srl_replay_sample.argtypes = [T, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     cdll.srl_replay_update.restype = c_int
     cdll.srl_replay_update.argtypes = [T, c_int, c_void_p, c_void_p, c_double, c_float, c_void_p]
+    S = POINTER(SrlSacNets)
+    cdll.srl_sac_arena_floats.restype = c_size_t
+    cdll.srl_sac_arena_floats.argtypes = [c_int, c_int]
+    cdll.srl_sac_workspace_bytes.restype = c_size_t
+    cdll.srl_sac_workspace_bytes.argtypes = [c_int, c_int, c_int]
+    cdll.srl_sac_act.restype = c_int
+    cdll.srl_sac_act.argtypes = [S, c_int, c_void_p, c_int, c_void_p, c_uint64, c_void_p, c_void_p]
+    cdll.srl_sac_store.restype = c_int
+    cdll.srl_sac_store.argtypes = [c_int, c_int, c_int, c_int] + [c_void_p] * 12
+    cdll.srl_sac_prepare.restype = c_int
+    cdll.srl_sac_prepare.argtypes = [S, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_float, c_float,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_sac_grad.restype = c_int
+    cdll.srl_sac_grad.argtypes = [S, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_sac_adam.restype = c_int
+    cdll.srl_sac_adam.argtypes = [S, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_int, c_float, c_void_p]
     return cdll
 
 
@@ -384,3 +406,125 @@ class FusedReplay(object):
     def update(self, batch, idx, td, eps, stream=None):
         rc = self._lib.srl_replay_update(byref(self.struct), int(batch), idx.data_ptr(), td.data_ptr(), self.alpha, float(eps), stream)
         self._library.check(rc, "srl_replay_update")
+
+
+# ---- SAC (include/srl_policy.h: srl_sac_*; rl_baselines/sac.py) ----
+
+class _FusedSAC(object):
+    """The library and the ``srl_sac_nets`` of an ``rl_baselines.sac.SACNets`` (its parameter arena and target, live on a CUDA device)."""
+
+    def __init__(self, library, nets):
+        self._lib = bind(library.lib)
+        self._library = library
+        if nets.arena.device.type != "cuda":
+            raise ValueError("%s needs the networks on a CUDA device (there is no CPU fallback)" % type(self).__name__)
+        if int(self._lib.srl_sac_arena_floats(nets.obs_dim, nets.act_dim)) != nets.arena.numel():
+            raise ValueError("%s: the arena of %d floats is not the layout of srl_sac_arena_floats(%d, %d)" % (type(self).__name__, nets.arena.numel(), nets.obs_dim, nets.act_dim))
+        s = SrlSacNets()
+        s.struct_size = ctypes.sizeof(SrlSacNets)
+        s.obs_dim, s.act_dim, s.arena, s.target = nets.obs_dim, nets.act_dim, nets.arena.data_ptr(), nets.target.data_ptr()
+        self.struct, self.nets, self.dev = s, nets, nets.arena.device
+
+    def _check(self, rc, name):
+        self._library.check(rc, name)
+
+
+class FusedSACAct(_FusedSAC):
+    """``srl_sac_act``: the action of an env batch, ``mode`` 0 sample, 1 ``tanh(mu)``, 2 uniform random; owns the sampling record ``rng``."""
+    SAMPLE, DETERMINISTIC, RANDOM = 0, 1, 2
+
+    def __init__(self, library, nets, seed, env_offset=0):
+        import torch
+        super().__init__(library, nets)
+        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=self.dev)
+        self.env_offset = int(env_offset)
+
+    def __call__(self, n, obs, act_out, mode=0, stream=None):
+        rc = self._lib.srl_sac_act(byref(self.struct), int(n), None if obs is None else obs.data_ptr(), int(mode), self.rng.data_ptr(), self.env_offset,
+                                   act_out.data_ptr(), stream)
+        self._check(rc, "srl_sac_act")
+
+
+class FusedSACStore(object):
+    """``srl_sac_store``: one lockstep step into ring row ``step % rows`` (the row read on the device), then ``obs <- new_obs`` and
+    ``step += 1``.  Owns ``step`` (int64 [2] {steps stored, 0})."""
+
+    def __init__(self, library, ring, device):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        self.ring = ring
+        self.rows, self.n, self.obs_dim = ring["obs"].shape
+        self.act_dim = ring["act"].shape[2]
+        self.step = torch.zeros(2, dtype=torch.int64, device=device)
+
+    def __call__(self, obs, act, rew, done, new_obs, stream=None):
+        r = self.ring
+        rc = self._lib.srl_sac_store(self.rows, self.n, self.obs_dim, self.act_dim, self.step.data_ptr(), obs.data_ptr(), act.data_ptr(), rew.data_ptr(),
+                                     done.data_ptr(), new_obs.data_ptr(), r["obs"].data_ptr(), r["act"].data_ptr(), r["rew"].data_ptr(), r["done"].data_ptr(),
+                                     r["next_obs"].data_ptr(), stream)
+        self._library.check(rc, "srl_sac_store")
+
+
+class FusedSACPrepare(_FusedSAC):
+    """``srl_sac_prepare``: sample indices, q_backup, v_backup, logp and the actor's head derivatives of ``batch`` samples; the gradient of
+    log_ent_coef goes to ``ent_grad`` (default: its entry of the gradient arena ``grad``).  Owns the sampling record ``rng`` and the outputs."""
+
+    def __init__(self, library, nets, ring, batch, seed, grad, workspace):
+        import torch
+        super().__init__(library, nets)
+        self.ring, self.batch = ring, int(batch)
+        self.rows, self.n = ring["obs"].shape[:2]
+        z = lambda *shape, dtype=torch.float32: torch.zeros(shape, dtype=dtype, device=self.dev)
+        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=self.dev)
+        self.idx, self.q_backup, self.v_backup, self.logp = z(batch, dtype=torch.int64), z(batch), z(batch), z(batch)
+        self.d_actor = z(batch, 2 * nets.act_dim)
+        self.ent_grad, self.workspace = grad[-1:], workspace
+
+    def __call__(self, step, gamma, ent_coef, target_entropy, stream=None):
+        """``ent_coef``: a float (fixed) or None ('auto': alpha = exp(log_ent_coef), read on the device)."""
+        r = self.ring
+        rc = self._lib.srl_sac_prepare(byref(self.struct), self.rows, self.n, step.data_ptr(), r["obs"].data_ptr(), r["act"].data_ptr(), r["rew"].data_ptr(),
+                                       r["done"].data_ptr(), r["next_obs"].data_ptr(), self.batch, float(gamma), int(ent_coef is None),
+                                       0.0 if ent_coef is None else float(ent_coef), float(target_entropy), self.rng.data_ptr(), self.idx.data_ptr(),
+                                       self.q_backup.data_ptr(), self.v_backup.data_ptr(), self.logp.data_ptr(), self.d_actor.data_ptr(),
+                                       self.ent_grad.data_ptr(), self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._check(rc, "srl_sac_prepare")
+
+
+class FusedSACGrad(_FusedSAC):
+    """``srl_sac_grad``: the weight gradients of the actor, qf1, qf2 and vf into the gradient arena ``grad`` (every entry but log_ent_coef's)
+    from what :class:`FusedSACPrepare` left.  ``workspace(...)`` sizes the scratch both share."""
+
+    @staticmethod
+    def workspace(library, nets, batch):
+        import torch
+        nbytes = int(bind(library.lib).srl_sac_workspace_bytes(nets.obs_dim, nets.act_dim, int(batch)))
+        if nbytes <= 0:
+            raise ValueError("srl_sac_workspace_bytes: unsupported shape")
+        return torch.zeros(nbytes, dtype=torch.uint8, device=nets.arena.device)
+
+    def __call__(self, prep, grad, stream=None):
+        r = prep.ring
+        rc = self._lib.srl_sac_grad(byref(self.struct), prep.n, r["obs"].data_ptr(), r["act"].data_ptr(), prep.batch, prep.idx.data_ptr(),
+                                    prep.q_backup.data_ptr(), prep.v_backup.data_ptr(), prep.d_actor.data_ptr(), grad.data_ptr(), prep.workspace.data_ptr(),
+                                    prep.workspace.numel(), stream)
+        self._check(rc, "srl_sac_grad")
+
+
+class FusedSACAdam(_FusedSAC):
+    """``srl_sac_adam``: TF1 Adam over the whole arena and the Polyak update of the target in one launch.  Owns the slots ``m``, ``v``,
+    TF's ``beta_power`` {beta1^t, beta2^t} (from {beta1, beta2}) and the learning rate ``lr`` (float32 [1])."""
+
+    def __init__(self, library, nets, beta1=0.9, beta2=0.999, epsilon=1e-8, tau=0.005):
+        import torch
+        super().__init__(library, nets)
+        self.m, self.v = torch.zeros_like(nets.arena), torch.zeros_like(nets.arena)
+        self.beta_power = torch.tensor([beta1, beta2], dtype=torch.float32, device=self.dev)
+        self.lr = torch.zeros(1, dtype=torch.float32, device=self.dev)
+        self.beta1, self.beta2, self.epsilon, self.tau = float(beta1), float(beta2), float(epsilon), float(tau)
+
+    def __call__(self, grad, polyak=True, stream=None):
+        rc = self._lib.srl_sac_adam(byref(self.struct), grad.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self.lr.data_ptr(), self.beta_power.data_ptr(),
+                                    self.beta1, self.beta2, self.epsilon, int(bool(polyak)), self.tau, stream)
+        self._check(rc, "srl_sac_adam")
