@@ -4,8 +4,8 @@ as the reference trains it through ``rl_baselines/rl_algorithm/ddpg.py``.  That 
 1e-4, critic_lr 1e-3, gamma 0.99, reward_scale 1, nb_rollout_steps 100, nb_train_steps 100, nb_eval_steps 50 (no eval env: no effect),
 batch_size ``--batch-size``, no observation / return normalisation, no popart, clip_norm None, and the action noise of ``--noise-action``
 (none, normal or Ornstein-Uhlenbeck, sigma ``--noise-action-sigma``); ``--hyperparam`` overrides them, ``noise_action`` and
-``noise_action_sigma`` there taking precedence over the flags.  Restated in PyTorch next to rl_baselines/sac.py, whose batched rule, replay
-ring and run helpers (rl_baselines/ppo2.py) it uses.
+``noise_action_sigma`` there taking precedence over the flags.  Restated in PyTorch next to rl_baselines/sac.py, whose batched rule and
+replay-ring loop (rl_baselines/offpolicy.py) it shares.
 
 RECALLED from stable-baselines 2.5, not checked against an installed copy (none can be installed here; include/srl_policy.h): tau 0.001;
 memory_limit 100 (the ring's default rows; the reference's ``--memory-limit`` is parsed and never passed to the model); observation_range
@@ -31,9 +31,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from rl_baselines.ppo2 import (RunLog, RunningNorm, allreduce_mean_gradients, first_observation, make_run, merge_running_moments, phase_timer,
-                               write_run_files)
-from rl_baselines.sac import ring_bytes
+from rl_baselines import offpolicy
+from rl_baselines.ppo2 import allreduce_mean_gradients
 
 MEMORY_LIMIT = 100                         # stable-baselines 2.5 DDPG's memory_limit (RECALLED): the default ring rows
 DDPG_DEFAULTS = dict(critic_l2_reg=1e-2, actor_lr=1e-4, critic_lr=1e-3, gamma=0.99, reward_scale=1.0, nb_rollout_steps=100, nb_train_steps=100,
@@ -165,12 +164,11 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     """DDPG.learn on a BatchedSRLVecEnv (module docstring); the signature and return value of rl_baselines.sac.train: a history of
     (timesteps, mean episode return, fps), one entry per cycle of ``nb_rollout_steps`` lockstep steps.
 
-    The steps run in blocks of G = nb_rollout_steps lockstep steps, or 2 nb_rollout_steps when that is odd and the blocks are captured
-    (MobileRobot's state double buffer needs an even number of simulator launches per graph replay).  ``cuda_graph`` (fused, single process, no ``phase_times``): every
-    full block after the first is ONE CUDA graph replay, the same graph for every block -- the ring row, the sampling counters, the OU state,
-    the step count and the learning rates are all read on the device.  The first block (it warms every kernel up) and a short last block run
-    the same launches eagerly.  ``phase_times``: a dict that accumulates the wall time of ``collect`` / ``prepare`` / ``gradient`` /
-    ``optimise``, synchronising between them (eager)."""
+    The steps run in rl_baselines.offpolicy.learn's blocks of G = nb_rollout_steps lockstep steps, or 2 nb_rollout_steps when that is odd
+    and the blocks are captured (MobileRobot's state double buffer needs an even number of simulator launches per graph replay).
+    ``cuda_graph`` (fused, single process, no ``phase_times``): every full block after the first is one graph replay (the OU state, the step
+    count and the learning rates are read on the device).  ``phase_times``: a dict that accumulates the wall time of ``collect`` /
+    ``prepare`` / ``gradient`` / ``optimise``, synchronising between them (eager)."""
     hp = dict(DDPG_DEFAULTS); hp.update(hyperparams or {})
     if dict(env_kwargs or {}).get("is_discrete", True):
         raise ValueError(DISCRETE_ERROR)
@@ -180,161 +178,60 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
         raise ValueError("noise_action must be one of %s (got %r)" % (sorted(NOISE_MODES), hp["noise_action"]))
     mode, sigma = NOISE_MODES[hp["noise_action"]], float(hp["noise_action_sigma"])
     torch.manual_seed(seed)
-    run = make_run("ddpg", env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, [fused],
-                   network=lambda width, env: DDPGNets(width, env.action_space.shape[0]))
-    env, on_gpu, dev, nets, dist, rank, world, K, W = run.env, run.on_gpu, run.dev, run.policy, run.dist, run.rank, run.world, run.K, run.W
-    nets.sync_target()                                        # after make_run's broadcast: every rank starts from one network
-    A = nets.act_dim
-    if fused is None:
-        fused = on_gpu
-    if fused and not on_gpu:
-        raise ValueError("fused=True needs the CUDA library (there is no CPU fallback)")
-    N, R, rows = num_envs, hp["nb_rollout_steps"], hp["buffer_size"]
-    B = hp["batch_size"] * N
-    n_steps = max(1, int(num_timesteps) // (N * world))
-    use_graph = bool(cuda_graph and fused and dist is None and phase_times is None)
-    G = 2 * R if R % 2 and use_graph else R
-    if on_gpu:                                                # before the ring or any step buffer is allocated
-        nbytes = ring_bytes(rows, N, W, A) + step_bytes(B, W, A, torch.cuda.get_device_properties(dev).multi_processor_count)
-        free, _ = torch.cuda.mem_get_info(dev)
-        if nbytes > free:
-            env.close()
-            raise ValueError("the replay ring of --buffer-size %d rows x %d envs and the gradient step's buffers need %.2f GB and the device has "
-                             "%.2f GB free: lower --buffer-size or --num-cpu" % (rows, N, nbytes / 1e9, free / 1e9))
-    norm = RunningNorm(W, dev)
-    write_run_files(run, log_dir, num_timesteps, seed, hp)
-    obs, stack = first_observation(run, norm)
-    z = lambda *shape, dtype=torch.float32: torch.zeros(shape, device=dev, dtype=dtype)
-    ring = dict(obs=z(rows, N, W), next_obs=z(rows, N, W), act=z(rows, N, A), rew=z(rows, N), done=z(rows, N, dtype=torch.uint8))
-    flat = {k: v.reshape((rows * N,) + v.shape[2:]) for k, v in ring.items()}
-    block = dict(done=z(G, N), ep_ret=z(G, N), ep_len=z(G, N, dtype=torch.int32))
-    grad = torch.zeros_like(nets.arena.data)
-    nets.arena.grad = grad                                   # the gradient arena, what allreduce_mean_gradients averages
-    done_s = z(N, dtype=torch.uint8)                          # the previous step's done flags (the OU reset)
-    if fused:
-        from srl_sim.policy import FusedDDPGAct, FusedDDPGAdam, FusedDDPGGrad, FusedDDPGPrepare, FusedPolicy, FusedSACStore
+    ctx = offpolicy.setup("ddpg", DDPGNets, env_id, num_envs, num_timesteps, seed, env_kwargs, log_dir, device, hp, verbose, fused, cuda_graph,
+                          phase_times, prefetch_resets, episode_window, num_stack, step_bytes)
+    env, dev, nets, dist, world, N, A, B, flat, grad, tick = ctx.env, ctx.dev, ctx.nets, ctx.dist, ctx.world, ctx.N, ctx.A, ctx.B, ctx.flat, ctx.grad, ctx.tick
+    R = hp["nb_rollout_steps"]
+    if ctx.fused:
+        from srl_sim.policy import FusedDDPGAct, FusedDDPGAdam, FusedDDPGGrad, FusedDDPGPrepare
         lib = env.backend.library
-        from rl_baselines.ppo2 import MlpPolicy
-        # its filter launches only (they read the width and the filter state); DDPG's networks are not an MlpPolicy
-        ffilter = FusedPolicy(lib, MlpPolicy(W, action_dim=A).to(dev), norm.state, seed=seed, env_offset=rank * N, clip=norm.clip, eps=norm.eps)
-        fact = FusedDDPGAct(lib, nets, N, seed=seed, sigma=sigma, theta=OU_THETA, dt=OU_DT, env_offset=rank * N)
-        fstore = FusedSACStore(lib, ring, dev)
-        fprep = FusedDDPGPrepare(lib, nets, ring, B, seed + 1 + rank)
+        fact = FusedDDPGAct(lib, nets, N, seed=seed, sigma=sigma, theta=OU_THETA, dt=OU_DT, env_offset=ctx.rank * N)
+        fprep = FusedDDPGPrepare(lib, nets, ctx.ring, B, seed + 1 + ctx.rank)
         fgrad = FusedDDPGGrad(lib, nets, B, hp["critic_l2_reg"])
         fopt = FusedDDPGAdam(lib, nets, hp["actor_lr"], hp["critic_lr"], hp["tau"], ADAM_BETA1, ADAM_BETA2, ADAM_EPS)
         m, v, t_adam, ou = fopt.m, fopt.v, fopt.t, fact.ou
-        act_dev, rew_s, new_obs = z(N, A), z(N), z(N, W)
-        obs_cur = obs.contiguous()
     else:
-        m, v, t_adam, ou = torch.zeros_like(grad), torch.zeros_like(grad), torch.zeros(1, dtype=torch.int64), z(N, A)
-        obs_cur = obs
-    if run.prefetch_resets and on_gpu:
-        env.sim.prefetch_resets(stream=env.backend.stream())
-    tick = phase_timer(phase_times, on_gpu)
-    stats = dict(grad_steps=0, graph_replays=0, graphs=0)
+        m, v, t_adam, ou = torch.zeros_like(grad), torch.zeros_like(grad), torch.zeros(1, dtype=torch.int64), torch.zeros(N, A, device=dev)
 
-    def env_step(t, k):
-        st = env.backend.stream()
-        with torch.no_grad():
-            if fused:
-                fact(N, obs_cur, done_s, act_dev, mode=mode, stream=st)
-                env.sim.step(act_dev, None, env._obs, rew_s, done_s, block["ep_ret"][k], block["ep_len"][k], stream=st)
-                if K > 1:
-                    ffilter.stack_filter(N, env._obs, done_s, stack, new_obs, update=True, stream=st)
-                else:
-                    ffilter.filter(N, env._obs, new_obs, update=True, stream=st)
-                fstore(obs_cur, act_dev, rew_s, done_s, new_obs, stream=st)          # ring row t % rows, then obs_cur <- new_obs
-                block["done"][k].copy_(done_s)
-                return
-            row = t % rows
-            a = nets.act(obs_cur)
-            if mode == NOISE_MODES["normal"]:
-                a = a + sigma * torch.randn(N, A, device=dev)
-            elif mode == NOISE_MODES["ou"]:
-                a = a + ou_step(ou, torch.randn(N, A, device=dev), done_s, sigma)
-            a = torch.clamp(a, -1.0, 1.0)
-            ring["obs"][row].copy_(obs_cur); ring["act"][row].copy_(a)
-            env.step_tensors(a.contiguous())
-            ring["rew"][row].copy_(run.e_rew); ring["done"][row].copy_(run.e_done); done_s.copy_(run.e_done)
-            block["done"][k].copy_(run.e_done); block["ep_ret"][k].copy_(run.e_ep_ret); block["ep_len"][k].copy_(run.e_ep_len)
-            if K > 1:                                        # VecFrameStack.step
-                stack.copy_(torch.where(run.e_done.bool()[:, None], 0.0, torch.roll(stack, -run.D, 1)))
-                stack[:, W - run.D:].copy_(run.e_obs)
-                ring["next_obs"][row].copy_(norm(stack))
-            else:
-                ring["next_obs"][row].copy_(norm(run.e_obs))
-            obs_cur.copy_(ring["next_obs"][row])
-
-    def gradient_step(t):
-        st = env.backend.stream()
-        if fused:
-            t_ph = tick()
-            fprep(fstore.step, hp["gamma"], hp["reward_scale"], stream=st)
-            t_ph = tick("prepare", t_ph)
-            fgrad(fprep, grad, stream=st)
-            if dist is not None:
-                allreduce_mean_gradients([nets.arena], dist, world)
-            t_ph = tick("gradient", t_ph)
-            fopt(grad, stream=st)
-            tick("optimise", t_ph)
+    def act(random_action):
+        if ctx.fused:
+            fact(N, ctx.obs, ctx.done_s, ctx.act_dev, mode=mode, stream=env.backend.stream())
             return
-        t_ph = tick()
-        size = min(t + 1, rows) * N
-        ix = torch.randint(0, size, (B,), device=dev)
-        L = ddpg_losses(nets, flat["obs"][ix], flat["act"][ix], flat["rew"][ix], flat["next_obs"][ix], flat["done"][ix].float(), hp["gamma"],
-                        hp["reward_scale"], hp["critic_l2_reg"])
+        a = nets.act(ctx.obs)
+        if mode == NOISE_MODES["normal"]:
+            a = a + sigma * torch.randn(N, A, device=dev)
+        elif mode == NOISE_MODES["ou"]:
+            a = a + ou_step(ou, torch.randn(N, A, device=dev), ctx.done_s, sigma)        # ctx.done_s: the previous step's done flags
+        ctx.act_dev.copy_(torch.clamp(a, -1.0, 1.0))
+
+    def gradient_step(t, polyak):                          # polyak is always True: the target update follows every gradient step
+        st, t_ph = env.backend.stream(), tick()
+        if ctx.fused:
+            fprep(ctx.fstore.step, hp["gamma"], hp["reward_scale"], stream=st)
+        else:
+            ix = torch.randint(0, min(t + 1, ctx.rows) * N, (B,), device=dev)
+            L = ddpg_losses(nets, flat["obs"][ix], flat["act"][ix], flat["rew"][ix], flat["next_obs"][ix], flat["done"][ix].float(), hp["gamma"],
+                            hp["reward_scale"], hp["critic_l2_reg"])
         t_ph = tick("prepare", t_ph)
-        grad.copy_(torch.autograd.grad(L["total"], nets.arena)[0])
+        if ctx.fused:
+            fgrad(fprep, grad, stream=st)
+        else:
+            grad.copy_(torch.autograd.grad(L["total"], nets.arena)[0])
         if dist is not None:
             allreduce_mean_gradients([nets.arena], dist, world)
         t_ph = tick("gradient", t_ph)
-        mpi_adam_polyak(nets, grad, m, v, t_adam, hp["actor_lr"], hp["critic_lr"], hp["tau"])
+        if ctx.fused:
+            fopt(grad, stream=st)
+        else:
+            mpi_adam_polyak(nets, grad, m, v, t_adam, hp["actor_lr"], hp["critic_lr"], hp["tau"])
         tick("optimise", t_ph)
 
-    def run_block(t0, steps):
-        for k in range(steps):
-            t = t0 + k
-            t_ph = tick()
-            env_step(t, k)
-            tick("collect", t_ph)
-            for _ in range(cadence(t, hp)):
-                if stats["grad_steps"] == 0:                 # what a test needs to redo the first gradient step
-                    train.last_before_first_step = dict(arena=nets.arena.detach().clone(), target=nets.target.clone(), m=m.clone(), v=v.clone(),
-                                                        t=t_adam.clone())
-                gradient_step(t)
-                stats["grad_steps"] += 1
-
-    graph = None
-    log = RunLog(run, norm, log_dir, max(1, 200 // (R * N * world)), episode_window, verbose)
-    log.start()
-    n_cycles = (n_steps + R - 1) // R
-    t0, c_i = 0, 0
-    while t0 < n_steps:
-        steps = min(G, n_steps - t0)
-        prior = (norm.mean.clone(), norm.var.clone(), norm.count.clone()) if dist is not None else None
-        if use_graph and stats["grad_steps"] > 0 and steps == G:
-            if graph is None:
-                graph, counts = torch.cuda.CUDAGraph(), dict(stats)
-                with torch.cuda.graph(graph):                  # capture records the launches only: nothing advances
-                    run_block(t0, G)
-                stats.update(counts, graphs=1)
-            graph.replay()
-            stats["graph_replays"] += 1
-            stats["grad_steps"] += sum(cadence(t, hp) for t in range(t0, t0 + G))
-        else:
-            run_block(t0, steps)
-        if dist is not None:
-            merge_running_moments(norm, prior, dist.all_reduce, world)
-        for k0 in range(0, steps, R):
-            n = min(R, steps - k0)
-            log.episodes(block["done"][k0:k0 + n], block["ep_ret"][k0:k0 + n], block["ep_len"][k0:k0 + n])
-            c_i += 1
-            log.end_update(c_i, n_cycles, (t0 + k0 + n) * N * world, print_every=max(1, n_cycles // 20))
-        t0 += steps
-    log.finish()
-    env.close()
+    # Every block starts at a multiple of R, so a full block has its gradient steps at its steps R - 1 (and 2 R - 1) and no random action:
+    # every full block after the first gradient step is the captured one (tests/test_ddpg_cpu.py::test_cadence).
+    log, stats = offpolicy.learn(ctx, R, 2 * R if R % 2 and ctx.use_graph else R, lambda t: (False, [True] * cadence(t, hp)), act, gradient_step,
+                                 dict(m=m, v=v, t=t_adam))
     train.best_mean_reward, train.n_saved, train.stats = log.best_mean_reward, log.n_saved, stats
-    train.last_nets, train.last_norm, train.last_ring, train.last_grad = nets, norm, ring, grad
-    train.last_adam, train.last_ou = (m, v, t_adam), ou
-    train.last_fused = dict(store=fstore, prepare=fprep, act=fact) if fused else None
+    train.last_nets, train.last_norm, train.last_ring, train.last_grad = nets, ctx.norm, ctx.ring, grad
+    train.last_adam, train.last_ou, train.last_before_first_step = (m, v, t_adam), ou, ctx.before_first_step
+    train.last_fused = dict(store=ctx.fstore, prepare=fprep, act=fact) if ctx.fused else None
     return log.history

@@ -232,9 +232,9 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     for p in params:
         p.grad = torch.zeros_like(p)
     if fused:
-        from srl_sim.policy import FusedClipAdam, FusedDQNAct, FusedDQNGrad, FusedDQNTarget, FusedPolicy, FusedReplay
+        from srl_sim.policy import FusedClipAdam, FusedDQNAct, FusedDQNGrad, FusedDQNTarget, FusedObsFilter, FusedReplay
         lib = env.backend.library
-        ffilter = FusedPolicy(lib, qnet, norm.state, seed=seed, env_offset=rank * N, clip=norm.clip, eps=norm.eps)    # its filter launches only
+        ffilter = FusedObsFilter(lib, norm.state, clip=norm.clip, eps=norm.eps)
         fact = FusedDQNAct(lib, qnet, seed=seed, env_offset=rank * N)
         ftarget = FusedDQNTarget(lib, qnet, target)
         fgrad = FusedDQNGrad(lib, qnet, B)

@@ -3,8 +3,8 @@ SAC consumer of the batched simulator: stable-baselines 2.5's ``SAC`` with its `
 through ``rl_baselines/rl_algorithm/sac.py``.  That file passes only ``--hyperparam`` values to the model (its ``--ent-coef`` and
 ``--batch-size`` are parsed and never used), so the library's defaults apply: gamma 0.99, learning_rate 3e-4 (constant), buffer_size 50 000,
 learning_starts 100, train_freq 1, batch_size 64, tau 0.005, ent_coef 'auto' (log_ent_coef from 0, target_entropy = -action_dim),
-target_update_interval 1, gradient_steps 1.  Restated in PyTorch next to rl_baselines/deepq.py, whose batched rule it follows and whose
-run helpers (rl_baselines/ppo2.py) it imports.
+target_update_interval 1, gradient_steps 1.  Restated in PyTorch next to rl_baselines/deepq.py, whose batched rule it follows; the replay-ring
+loop is rl_baselines/offpolicy.py, shared with DDPG.
 
 RECALLED from stable-baselines 2.5, not checked against an installed copy (none can be installed here; include/srl_policy.h): the defaults
 above; the networks (layers [64, 64], ReLU, glorot-uniform weights and zero biases; an actor trunk with separate ``mu`` and ``log_std`` heads,
@@ -32,8 +32,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from rl_baselines.ppo2 import (RunLog, RunningNorm, allreduce_mean_gradients, first_observation, make_run, merge_running_moments, phase_timer,
-                               write_run_files)
+from rl_baselines import offpolicy
+from rl_baselines.ppo2 import allreduce_mean_gradients
 
 SAC_DEFAULTS = dict(gamma=0.99, learning_rate=3e-4, buffer_size=50000, learning_starts=100, train_freq=1, batch_size=64, tau=0.005,
                     ent_coef="auto", target_update_interval=1, gradient_steps=1)          # stable-baselines 2.5 SAC (RECALLED)
@@ -182,11 +182,6 @@ def cadence(t, hp):
     return random_action, [(t + g) % hp["target_update_interval"] == 0 for g in range(hp["gradient_steps"])]
 
 
-def ring_bytes(rows, n_envs, W, A):
-    """Device bytes of the replay ring: obs and next_obs f32[rows, N, W], act f32[rows, N, A], rew f32 and done u8 [rows, N]."""
-    return int(rows) * int(n_envs) * (4 * (2 * W + A + 1) + 1)
-
-
 def step_bytes(batch, W, A, sms):
     """Device bytes of one gradient step's buffers beside the ring: idx i64, q_backup / v_backup / logp f32 and d_actor f32[2A] per sample,
     and srl_sac_grad's per-CTA partial gradients (at most one CTA per SM)."""
@@ -198,185 +193,67 @@ def train(env_id, num_envs, num_timesteps, seed=0, env_kwargs=None, log_dir=None
     """SAC.learn on a BatchedSRLVecEnv (module docstring); the signature and return value of rl_baselines.deepq.train: a history of
     (timesteps, mean episode return, fps), one entry per ``train_freq`` lockstep steps.
 
-    The steps run in blocks of G = train_freq lockstep steps, or 2 train_freq when train_freq is odd (MobileRobot's state double buffer needs
-    an even number of simulator launches per graph replay).  ``cuda_graph`` (fused, single process, no ``phase_times``): a block with no
-    random action and every gradient step taken is ONE CUDA graph replay, the same graph for every such block -- the ring row, the sampling
-    counters, the learning rate and log_ent_coef are all read on the device.  The random-action phase, the first block with gradient steps
-    (it warms every kernel up) and a short last block run the same launches eagerly.  ``phase_times``: a dict that accumulates the wall time
-    of ``collect`` / ``prepare`` / ``gradient`` / ``optimise``, synchronising between them (eager)."""
+    The steps run in rl_baselines.offpolicy.learn's blocks of G = train_freq lockstep steps, or 2 train_freq when train_freq is odd
+    (MobileRobot's state double buffer needs an even number of simulator launches per graph replay).  ``cuda_graph`` (fused, single process,
+    no ``phase_times``): a block with no random action and every gradient step taken is one graph replay (the learning rate and log_ent_coef
+    are read on the device).  ``phase_times``: a dict that accumulates the wall time of ``collect`` / ``prepare`` / ``gradient`` /
+    ``optimise``, synchronising between them (eager)."""
     hp = dict(SAC_DEFAULTS); hp.update(hyperparams or {})
     if dict(env_kwargs or {}).get("is_discrete", True):
         raise ValueError(DISCRETE_ERROR)
     torch.manual_seed(seed)
-    run = make_run("sac", env_id, num_envs, seed, env_kwargs, device, prefetch_resets, num_stack, [fused],
-                   network=lambda width, env: SACNets(width, env.action_space.shape[0]))
-    env, on_gpu, dev, nets, dist, rank, world, K, W = run.env, run.on_gpu, run.dev, run.policy, run.dist, run.rank, run.world, run.K, run.W
-    nets.sync_target()                                        # after make_run's broadcast: every rank starts from one vf
-    A = nets.act_dim
-    if fused is None:
-        fused = on_gpu
-    if fused and not on_gpu:
-        raise ValueError("fused=True needs the CUDA library (there is no CPU fallback)")
-    N, F, rows = num_envs, hp["train_freq"], hp["buffer_size"]
-    G = F if F % 2 == 0 else 2 * F
-    B = hp["batch_size"] * N
-    auto_ent = hp["ent_coef"] == "auto"
-    ent_coef = None if auto_ent else float(hp["ent_coef"])
+    ctx = offpolicy.setup("sac", SACNets, env_id, num_envs, num_timesteps, seed, env_kwargs, log_dir, device, hp, verbose, fused, cuda_graph,
+                          phase_times, prefetch_resets, episode_window, num_stack, step_bytes)
+    env, dev, nets, dist, world, N, A, B, flat, grad, tick = ctx.env, ctx.dev, ctx.nets, ctx.dist, ctx.world, ctx.N, ctx.A, ctx.B, ctx.flat, ctx.grad, ctx.tick
+    F = hp["train_freq"]
+    ent_coef = None if hp["ent_coef"] == "auto" else float(hp["ent_coef"])
     target_entropy = -float(A)
-    n_steps = max(1, int(num_timesteps) // (N * world))
-    use_graph = bool(cuda_graph and fused and dist is None and phase_times is None)
-    if on_gpu:                                                # before the ring or any step buffer is allocated
-        nbytes = ring_bytes(rows, N, W, A) + step_bytes(B, W, A, torch.cuda.get_device_properties(dev).multi_processor_count)
-        free, _ = torch.cuda.mem_get_info(dev)
-        if nbytes > free:
-            env.close()
-            raise ValueError("the replay ring of --buffer-size %d rows x %d envs and the gradient step's buffers need %.2f GB and the device has "
-                             "%.2f GB free: lower --buffer-size or --num-cpu" % (rows, N, nbytes / 1e9, free / 1e9))
-    norm = RunningNorm(W, dev)
-    write_run_files(run, log_dir, num_timesteps, seed, hp)
-    obs, stack = first_observation(run, norm)
-    z = lambda *shape, dtype=torch.float32: torch.zeros(shape, device=dev, dtype=dtype)
-    ring = dict(obs=z(rows, N, W), next_obs=z(rows, N, W), act=z(rows, N, A), rew=z(rows, N), done=z(rows, N, dtype=torch.uint8))
-    flat = {k: v.reshape((rows * N,) + v.shape[2:]) for k, v in ring.items()}
-    block = dict(done=z(G, N), ep_ret=z(G, N), ep_len=z(G, N, dtype=torch.int32))
-    grad = torch.zeros_like(nets.arena.data)
-    nets.arena.grad = grad                                   # the gradient arena, what allreduce_mean_gradients averages
-    if fused:
-        from srl_sim.policy import FusedPolicy, FusedSACAct, FusedSACAdam, FusedSACGrad, FusedSACPrepare, FusedSACStore
+    if ctx.fused:
+        from srl_sim.policy import FusedSACAct, FusedSACAdam, FusedSACGrad, FusedSACPrepare
         lib = env.backend.library
-        from rl_baselines.ppo2 import MlpPolicy
-        # its filter launches only (they read the width and the filter state); SAC's networks are not an MlpPolicy
-        ffilter = FusedPolicy(lib, MlpPolicy(W, action_dim=A).to(dev), norm.state, seed=seed, env_offset=rank * N, clip=norm.clip, eps=norm.eps)
-        fact = FusedSACAct(lib, nets, seed=seed, env_offset=rank * N)
-        fstore = FusedSACStore(lib, ring, dev)
+        fact = FusedSACAct(lib, nets, seed=seed, env_offset=ctx.rank * N)
         workspace = FusedSACGrad.workspace(lib, nets, B)
-        fprep = FusedSACPrepare(lib, nets, ring, B, seed + 1 + rank, grad, workspace)
+        fprep = FusedSACPrepare(lib, nets, ctx.ring, B, seed + 1 + ctx.rank, grad, workspace)
         fgrad = FusedSACGrad(lib, nets)
         fopt = FusedSACAdam(lib, nets, ADAM_BETA1, ADAM_BETA2, ADAM_EPS, hp["tau"])
         fopt.lr.fill_(hp["learning_rate"])
         m, v, beta_power = fopt.m, fopt.v, fopt.beta_power
-        act_dev, rew_s, done_s, new_obs = z(N, A), z(N), z(N, dtype=torch.uint8), z(N, W)
-        obs_cur = obs.contiguous()
     else:
         m, v = torch.zeros_like(grad), torch.zeros_like(grad)
         beta_power = torch.tensor([ADAM_BETA1, ADAM_BETA2], dtype=torch.float32, device=dev)
-        obs_cur = obs
-    if run.prefetch_resets and on_gpu:
-        env.sim.prefetch_resets(stream=env.backend.stream())
-    tick = phase_timer(phase_times, on_gpu)
-    stats = dict(grad_steps=0, target_updates=0, graph_replays=0, graphs=0)
 
-    def env_step(t, k, random_action):
-        st = env.backend.stream()
-        with torch.no_grad():
-            if fused:
-                fact(N, obs_cur, act_dev, mode=FusedSACAct.RANDOM if random_action else FusedSACAct.SAMPLE, stream=st)
-                env.sim.step(act_dev, None, env._obs, rew_s, done_s, block["ep_ret"][k], block["ep_len"][k], stream=st)
-                if K > 1:
-                    ffilter.stack_filter(N, env._obs, done_s, stack, new_obs, update=True, stream=st)
-                else:
-                    ffilter.filter(N, env._obs, new_obs, update=True, stream=st)
-                fstore(obs_cur, act_dev, rew_s, done_s, new_obs, stream=st)          # ring row t % rows, then obs_cur <- new_obs
-                block["done"][k].copy_(done_s)
-                return
-            row = t % rows
-            a = torch.rand(N, A, device=dev) * 2 - 1 if random_action else nets.act(obs_cur)
-            ring["obs"][row].copy_(obs_cur); ring["act"][row].copy_(a)
-            env.step_tensors(a.contiguous())
-            ring["rew"][row].copy_(run.e_rew); ring["done"][row].copy_(run.e_done)
-            block["done"][k].copy_(run.e_done); block["ep_ret"][k].copy_(run.e_ep_ret); block["ep_len"][k].copy_(run.e_ep_len)
-            if K > 1:                                        # VecFrameStack.step
-                stack.copy_(torch.where(run.e_done.bool()[:, None], 0.0, torch.roll(stack, -run.D, 1)))
-                stack[:, W - run.D:].copy_(run.e_obs)
-                ring["next_obs"][row].copy_(norm(stack))
-            else:
-                ring["next_obs"][row].copy_(norm(run.e_obs))
-            obs_cur.copy_(ring["next_obs"][row])
+    def act(random_action):
+        if ctx.fused:
+            fact(N, ctx.obs, ctx.act_dev, mode=FusedSACAct.RANDOM if random_action else FusedSACAct.SAMPLE, stream=env.backend.stream())
+        else:
+            ctx.act_dev.copy_(torch.rand(N, A, device=dev) * 2 - 1 if random_action else nets.act(ctx.obs))
 
     def gradient_step(t, polyak):
-        st = env.backend.stream()
-        if fused:
-            t_ph = tick()
-            fprep(fstore.step, hp["gamma"], ent_coef, target_entropy, stream=st)
-            t_ph = tick("prepare", t_ph)
-            fgrad(fprep, grad, stream=st)
-            if dist is not None:
-                allreduce_mean_gradients([nets.arena], dist, world)
-            t_ph = tick("gradient", t_ph)
-            fopt(grad, polyak=polyak, stream=st)
-            tick("optimise", t_ph)
-            return
-        t_ph = tick()
-        size = min(t + 1, rows) * N
-        ix = torch.randint(0, size, (B,), device=dev)
-        eps = torch.randn(B, A, device=dev)
-        L = sac_losses(nets, flat["obs"][ix], flat["act"][ix], flat["rew"][ix], flat["next_obs"][ix], flat["done"][ix].float(), eps, hp["gamma"],
-                       ent_coef, target_entropy)
+        st, t_ph = env.backend.stream(), tick()
+        if ctx.fused:
+            fprep(ctx.fstore.step, hp["gamma"], ent_coef, target_entropy, stream=st)
+        else:
+            ix = torch.randint(0, min(t + 1, ctx.rows) * N, (B,), device=dev)
+            eps = torch.randn(B, A, device=dev)
+            L = sac_losses(nets, flat["obs"][ix], flat["act"][ix], flat["rew"][ix], flat["next_obs"][ix], flat["done"][ix].float(), eps,
+                           hp["gamma"], ent_coef, target_entropy)
         t_ph = tick("prepare", t_ph)
-        grad.copy_(torch.autograd.grad(L["total"], nets.arena)[0])
+        if ctx.fused:
+            fgrad(fprep, grad, stream=st)
+        else:
+            grad.copy_(torch.autograd.grad(L["total"], nets.arena)[0])
         if dist is not None:
             allreduce_mean_gradients([nets.arena], dist, world)
         t_ph = tick("gradient", t_ph)
-        adam_polyak(nets, grad, m, v, beta_power, hp["learning_rate"], hp["tau"], polyak)
+        if ctx.fused:
+            fopt(grad, polyak=polyak, stream=st)
+        else:
+            adam_polyak(nets, grad, m, v, beta_power, hp["learning_rate"], hp["tau"], polyak)
         tick("optimise", t_ph)
 
-    def run_block(t0, steps):
-        for k in range(steps):
-            t = t0 + k
-            random_action, targets = cadence(t, hp)
-            t_ph = tick()
-            env_step(t, k, random_action)
-            tick("collect", t_ph)
-            for polyak in targets:
-                if stats["grad_steps"] == 0:                 # what a test needs to redo the first gradient step
-                    train.last_before_first_step = dict(arena=nets.arena.detach().clone(), target=nets.target.clone(), m=m.clone(), v=v.clone(),
-                                                        beta_power=beta_power.clone())
-                gradient_step(t, polyak)
-                stats["grad_steps"] += 1
-                stats["target_updates"] += int(polyak)
-
-    def block_pattern(t0):
-        """The gradient steps (their target updates) at each step of the block at t0, or None when the block cannot be the graph's: a short
-        last block, or one with a random action or a skipped gradient step."""
-        if t0 + G > n_steps or t0 < hp["learning_starts"] or t0 + 1 < hp["batch_size"]:
-            return None
-        return [cadence(t, hp)[1] for t in range(t0, t0 + G)]
-
-    graph, graph_pattern, warmed = None, None, False
-    log = RunLog(run, norm, log_dir, max(1, 200 // (F * N * world)), episode_window, verbose)
-    log.start()
-    n_periods = (n_steps + F - 1) // F
-    t0, p_i = 0, 0
-    while t0 < n_steps:
-        steps = min(G, n_steps - t0)
-        prior = (norm.mean.clone(), norm.var.clone(), norm.count.clone()) if dist is not None else None
-        pat = block_pattern(t0) if use_graph and warmed else None
-        if pat is not None and (graph is None or pat == graph_pattern):
-            if graph is None:
-                graph, graph_pattern, counts = torch.cuda.CUDAGraph(), pat, dict(stats)
-                with torch.cuda.graph(graph):                  # capture records the launches only: nothing advances
-                    run_block(t0, G)
-                stats.update(counts, graphs=1)
-            graph.replay()
-            stats["graph_replays"] += 1
-            stats["grad_steps"] += sum(len(tg) for tg in pat)
-            stats["target_updates"] += sum(sum(tg) for tg in pat)
-        else:
-            run_block(t0, steps)
-            warmed = warmed or stats["grad_steps"] > 0
-        if dist is not None:
-            merge_running_moments(norm, prior, dist.all_reduce, world)
-        for k0 in range(0, steps, F):
-            n = min(F, steps - k0)
-            log.episodes(block["done"][k0:k0 + n], block["ep_ret"][k0:k0 + n], block["ep_len"][k0:k0 + n])
-            p_i += 1
-            log.end_update(p_i, n_periods, (t0 + k0 + n) * N * world, print_every=max(1, n_periods // 20))
-        t0 += steps
-    log.finish()
-    env.close()
+    log, stats = offpolicy.learn(ctx, F, F if F % 2 == 0 else 2 * F, lambda t: cadence(t, hp), act, gradient_step, dict(m=m, v=v, beta_power=beta_power))
     train.best_mean_reward, train.n_saved, train.stats = log.best_mean_reward, log.n_saved, stats
-    train.last_nets, train.last_norm, train.last_ring, train.last_grad = nets, norm, ring, grad
-    train.last_adam = (m, v, beta_power)
-    train.last_fused = dict(store=fstore, prepare=fprep, act=fact) if fused else None
+    train.last_nets, train.last_norm, train.last_ring, train.last_grad = nets, ctx.norm, ctx.ring, grad
+    train.last_adam, train.last_before_first_step = (m, v, beta_power), ctx.before_first_step
+    train.last_fused = dict(store=ctx.fstore, prepare=fprep, act=fact) if ctx.fused else None
     return log.history
-

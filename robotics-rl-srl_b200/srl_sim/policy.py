@@ -40,13 +40,8 @@ class SrlReplayTree(Structure):
                [(name, c_void_p) for name in ("sum", "min", "max_priority", "size", "stamp")]
 
 
-class SrlSacNets(Structure):
-    """struct srl_sac_nets (include/srl_policy.h)."""
-    _fields_ = [("struct_size", c_uint32), ("obs_dim", c_int32), ("act_dim", c_int32), ("reserved", c_int32), ("arena", c_void_p), ("target", c_void_p)]
-
-
-class SrlDdpgNets(Structure):
-    """struct srl_ddpg_nets (include/srl_policy.h)."""
+class SrlArenaNets(Structure):
+    """struct srl_sac_nets and struct srl_ddpg_nets (include/srl_policy.h: one layout)."""
     _fields_ = [("struct_size", c_uint32), ("obs_dim", c_int32), ("act_dim", c_int32), ("reserved", c_int32), ("arena", c_void_p), ("target", c_void_p)]
 
 
@@ -89,7 +84,7 @@ def bind(cdll):
     cdll.srl_replay_sample.argtypes = [T, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     cdll.srl_replay_update.restype = c_int
     cdll.srl_replay_update.argtypes = [T, c_int, c_void_p, c_void_p, c_double, c_float, c_void_p]
-    S = POINTER(SrlSacNets)
+    S = POINTER(SrlArenaNets)
     cdll.srl_sac_arena_floats.restype = c_size_t
     cdll.srl_sac_arena_floats.argtypes = [c_int, c_int]
     cdll.srl_sac_workspace_bytes.restype = c_size_t
@@ -105,19 +100,18 @@ def bind(cdll):
     cdll.srl_sac_grad.argtypes = [S, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
     cdll.srl_sac_adam.restype = c_int
     cdll.srl_sac_adam.argtypes = [S, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_int, c_float, c_void_p]
-    D = POINTER(SrlDdpgNets)
     cdll.srl_ddpg_arena_floats.restype = c_size_t
     cdll.srl_ddpg_arena_floats.argtypes = [c_int, c_int]
     cdll.srl_ddpg_workspace_bytes.restype = c_size_t
     cdll.srl_ddpg_workspace_bytes.argtypes = [c_int, c_int, c_int]
     cdll.srl_ddpg_act.restype = c_int
-    cdll.srl_ddpg_act.argtypes = [D, c_int, c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p]
+    cdll.srl_ddpg_act.argtypes = [S, c_int, c_void_p, c_int, c_float, c_float, c_float, c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p]
     cdll.srl_ddpg_prepare.restype = c_int
-    cdll.srl_ddpg_prepare.argtypes = [D, c_int, c_int] + [c_void_p] * 5 + [c_int, c_float, c_float] + [c_void_p] * 6
+    cdll.srl_ddpg_prepare.argtypes = [S, c_int, c_int] + [c_void_p] * 5 + [c_int, c_float, c_float] + [c_void_p] * 6
     cdll.srl_ddpg_grad.restype = c_int
-    cdll.srl_ddpg_grad.argtypes = [D, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_ddpg_grad.argtypes = [S, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_size_t, c_void_p]
     cdll.srl_ddpg_adam.restype = c_int
-    cdll.srl_ddpg_adam.argtypes = [D, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_double, c_void_p]
+    cdll.srl_ddpg_adam.argtypes = [S, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_double, c_void_p]
     return cdll
 
 
@@ -162,35 +156,24 @@ def policy_struct(policy):
     return s, tensors
 
 
-class FusedPolicy(object):
-    """The fused policy step + observation filter on the CUDA library, for one ``MlpPolicy`` and one env batch."""
+class FusedObsFilter(object):
+    """The VecNormalize observation filter on the CUDA library (``srl_obs_filter``; with a frame stack ``srl_obs_stack_filter``) over one
+    filter state: what every trainer's fused env step runs after the simulator step."""
 
-    def __init__(self, library, policy, filter_state, seed, env_offset=0, clip=10.0, eps=1e-8):
+    def __init__(self, library, filter_state, clip=10.0, eps=1e-8):
         """
         :param library: (srl_sim._abi.SimLibrary) the loaded CUDA library
-        :param policy: (rl_baselines.ppo2.MlpPolicy) on a CUDA device
-        :param filter_state: (torch.Tensor) float64 [2 * obs_dim + 1] on the same device: mean, var, count (updated in place)
-        :param seed: (int) key of the sampling streams; env ``i`` uses the stream (seed, env_offset + i)
+        :param filter_state: (torch.Tensor) float64 [2 * obs_dim + 1] on a CUDA device: mean, var, count (updated in place)
         """
         import torch
         self._lib = bind(library.lib)
         self._library = library
-        self.struct, self._keep = policy_struct(policy)
-        dev = policy.pi[0].weight.device
-        if dev.type != "cuda":
-            raise ValueError("FusedPolicy needs a policy on a CUDA device (there is no CPU fallback)")
-        if filter_state.dtype != torch.float64 or filter_state.numel() != 2 * self.struct.obs_dim + 1 or not filter_state.is_contiguous():
-            raise ValueError("filter_state must be a contiguous float64 tensor of 2 * obs_dim + 1 elements")
+        n = filter_state.numel()
+        if filter_state.device.type != "cuda" or filter_state.dtype != torch.float64 or n < 3 or n % 2 != 1 or not filter_state.is_contiguous():
+            raise ValueError("filter_state must be a contiguous float64 CUDA tensor of 2 * obs_dim + 1 elements")
         self.filter_state = filter_state
-        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=dev)   # {seed, step counter, arrivals}
-        self.env_offset, self.clip, self.eps = int(env_offset), float(clip), float(eps)
-        self.obs_dim, self.n_out, self.discrete = self.struct.obs_dim, self.struct.n_out, bool(self.struct.discrete)
-
-    def act(self, n, obs, act_env, logp, value, obs_buf=None, act_buf=None, stream=None):
-        rc = self._lib.srl_policy_act(byref(self.struct), int(n), obs.data_ptr(), self.rng.data_ptr(), self.env_offset,
-                                      None if obs_buf is None else obs_buf.data_ptr(), act_env.data_ptr(),
-                                      None if act_buf is None else act_buf.data_ptr(), logp.data_ptr(), value.data_ptr(), stream)
-        self._library.check(rc, "srl_policy_act")
+        self.obs_dim = (n - 1) // 2
+        self.clip, self.eps = float(clip), float(eps)
 
     def filter(self, n, obs_raw, obs_norm_out, update=True, stream=None):
         rc = self._lib.srl_obs_filter(int(n), self.obs_dim, obs_raw.data_ptr(), self.filter_state.data_ptr(), int(bool(update)),
@@ -207,6 +190,35 @@ class FusedPolicy(object):
         rc = self._lib.srl_obs_stack_filter(int(n), D, self.obs_dim // D, obs_raw.data_ptr(), None if done is None else done.data_ptr(), stack.data_ptr(),
                                             self.filter_state.data_ptr(), int(bool(update)), self.clip, self.eps, obs_norm_out.data_ptr(), stream)
         self._library.check(rc, "srl_obs_stack_filter")
+
+
+class FusedPolicy(FusedObsFilter):
+    """The fused policy step + observation filter on the CUDA library, for one ``MlpPolicy`` and one env batch."""
+
+    def __init__(self, library, policy, filter_state, seed, env_offset=0, clip=10.0, eps=1e-8):
+        """
+        :param library: (srl_sim._abi.SimLibrary) the loaded CUDA library
+        :param policy: (rl_baselines.ppo2.MlpPolicy) on a CUDA device
+        :param filter_state: (torch.Tensor) float64 [2 * obs_dim + 1] on the same device: mean, var, count (updated in place)
+        :param seed: (int) key of the sampling streams; env ``i`` uses the stream (seed, env_offset + i)
+        """
+        import torch
+        self.struct, self._keep = policy_struct(policy)
+        dev = policy.pi[0].weight.device
+        if dev.type != "cuda":
+            raise ValueError("FusedPolicy needs a policy on a CUDA device (there is no CPU fallback)")
+        if filter_state.numel() != 2 * self.struct.obs_dim + 1:
+            raise ValueError("filter_state must hold 2 * obs_dim + 1 elements for the policy's obs_dim %d" % self.struct.obs_dim)
+        super().__init__(library, filter_state, clip, eps)
+        self.rng = torch.tensor([int(seed) & 0x7FFFFFFFFFFFFFFF, 0, 0], dtype=torch.int64, device=dev)   # {seed, step counter, arrivals}
+        self.env_offset = int(env_offset)
+        self.n_out, self.discrete = self.struct.n_out, bool(self.struct.discrete)
+
+    def act(self, n, obs, act_env, logp, value, obs_buf=None, act_buf=None, stream=None):
+        rc = self._lib.srl_policy_act(byref(self.struct), int(n), obs.data_ptr(), self.rng.data_ptr(), self.env_offset,
+                                      None if obs_buf is None else obs_buf.data_ptr(), act_env.data_ptr(),
+                                      None if act_buf is None else act_buf.data_ptr(), logp.data_ptr(), value.data_ptr(), stream)
+        self._library.check(rc, "srl_policy_act")
 
 
 class FusedPPO2Grad(object):
@@ -427,20 +439,23 @@ class FusedReplay(object):
         self._library.check(rc, "srl_replay_update")
 
 
-# ---- SAC (include/srl_policy.h: srl_sac_*; rl_baselines/sac.py) ----
+# ---- SAC and DDPG (include/srl_policy.h: srl_sac_*, srl_ddpg_*; rl_baselines/sac.py, rl_baselines/ddpg.py) ----
 
-class _FusedSAC(object):
-    """The library and the ``srl_sac_nets`` of an ``rl_baselines.sac.SACNets`` (its parameter arena and target, live on a CUDA device)."""
+class _FusedArena(object):
+    """The library and the ``srl_sac_nets`` / ``srl_ddpg_nets`` of an ``rl_baselines.sac.SACNets`` or ``rl_baselines.ddpg.DDPGNets`` (its
+    parameter arena and target, live on a CUDA device), the arena's size checked against the subclass's ``_arena_floats`` export."""
+    _arena_floats = None
 
     def __init__(self, library, nets):
         self._lib = bind(library.lib)
         self._library = library
         if nets.arena.device.type != "cuda":
             raise ValueError("%s needs the networks on a CUDA device (there is no CPU fallback)" % type(self).__name__)
-        if int(self._lib.srl_sac_arena_floats(nets.obs_dim, nets.act_dim)) != nets.arena.numel():
-            raise ValueError("%s: the arena of %d floats is not the layout of srl_sac_arena_floats(%d, %d)" % (type(self).__name__, nets.arena.numel(), nets.obs_dim, nets.act_dim))
-        s = SrlSacNets()
-        s.struct_size = ctypes.sizeof(SrlSacNets)
+        if int(getattr(self._lib, self._arena_floats)(nets.obs_dim, nets.act_dim)) != nets.arena.numel():
+            raise ValueError("%s: the arena of %d floats is not the layout of %s(%d, %d)" % (type(self).__name__, nets.arena.numel(), self._arena_floats,
+                                                                                             nets.obs_dim, nets.act_dim))
+        s = SrlArenaNets()
+        s.struct_size = ctypes.sizeof(SrlArenaNets)
         s.obs_dim, s.act_dim, s.arena, s.target = nets.obs_dim, nets.act_dim, nets.arena.data_ptr(), nets.target.data_ptr()
         self.struct, self.nets, self.dev = s, nets, nets.arena.device
 
@@ -448,8 +463,9 @@ class _FusedSAC(object):
         self._library.check(rc, name)
 
 
-class FusedSACAct(_FusedSAC):
+class FusedSACAct(_FusedArena):
     """``srl_sac_act``: the action of an env batch, ``mode`` 0 sample, 1 ``tanh(mu)``, 2 uniform random; owns the sampling record ``rng``."""
+    _arena_floats = "srl_sac_arena_floats"
     SAMPLE, DETERMINISTIC, RANDOM = 0, 1, 2
 
     def __init__(self, library, nets, seed, env_offset=0):
@@ -485,9 +501,10 @@ class FusedSACStore(object):
         self._library.check(rc, "srl_sac_store")
 
 
-class FusedSACPrepare(_FusedSAC):
+class FusedSACPrepare(_FusedArena):
     """``srl_sac_prepare``: sample indices, q_backup, v_backup, logp and the actor's head derivatives of ``batch`` samples; the gradient of
     log_ent_coef goes to ``ent_grad`` (default: its entry of the gradient arena ``grad``).  Owns the sampling record ``rng`` and the outputs."""
+    _arena_floats = "srl_sac_arena_floats"
 
     def __init__(self, library, nets, ring, batch, seed, grad, workspace):
         import torch
@@ -511,9 +528,10 @@ class FusedSACPrepare(_FusedSAC):
         self._check(rc, "srl_sac_prepare")
 
 
-class FusedSACGrad(_FusedSAC):
+class FusedSACGrad(_FusedArena):
     """``srl_sac_grad``: the weight gradients of the actor, qf1, qf2 and vf into the gradient arena ``grad`` (every entry but log_ent_coef's)
     from what :class:`FusedSACPrepare` left.  ``workspace(...)`` sizes the scratch both share."""
+    _arena_floats = "srl_sac_arena_floats"
 
     @staticmethod
     def workspace(library, nets, batch):
@@ -531,9 +549,10 @@ class FusedSACGrad(_FusedSAC):
         self._check(rc, "srl_sac_grad")
 
 
-class FusedSACAdam(_FusedSAC):
+class FusedSACAdam(_FusedArena):
     """``srl_sac_adam``: TF1 Adam over the whole arena and the Polyak update of the target in one launch.  Owns the slots ``m``, ``v``,
     TF's ``beta_power`` {beta1^t, beta2^t} (from {beta1, beta2}) and the learning rate ``lr`` (float32 [1])."""
+    _arena_floats = "srl_sac_arena_floats"
 
     def __init__(self, library, nets, beta1=0.9, beta2=0.999, epsilon=1e-8, tau=0.005):
         import torch
@@ -549,30 +568,10 @@ class FusedSACAdam(_FusedSAC):
         self._check(rc, "srl_sac_adam")
 
 
-# ---- DDPG (include/srl_policy.h: srl_ddpg_*; rl_baselines/ddpg.py) ----
-
-class _FusedDDPG(object):
-    """The library and the ``srl_ddpg_nets`` of an ``rl_baselines.ddpg.DDPGNets`` (its parameter arena and targets, live on a CUDA device)."""
-
-    def __init__(self, library, nets):
-        self._lib = bind(library.lib)
-        self._library = library
-        if nets.arena.device.type != "cuda":
-            raise ValueError("%s needs the networks on a CUDA device (there is no CPU fallback)" % type(self).__name__)
-        if int(self._lib.srl_ddpg_arena_floats(nets.obs_dim, nets.act_dim)) != nets.arena.numel():
-            raise ValueError("%s: the arena of %d floats is not the layout of srl_ddpg_arena_floats(%d, %d)" % (type(self).__name__, nets.arena.numel(), nets.obs_dim, nets.act_dim))
-        s = SrlDdpgNets()
-        s.struct_size = ctypes.sizeof(SrlDdpgNets)
-        s.obs_dim, s.act_dim, s.arena, s.target = nets.obs_dim, nets.act_dim, nets.arena.data_ptr(), nets.target.data_ptr()
-        self.struct, self.nets, self.dev = s, nets, nets.arena.device
-
-    def _check(self, rc, name):
-        self._library.check(rc, name)
-
-
-class FusedDDPGAct(_FusedDDPG):
+class FusedDDPGAct(_FusedArena):
     """``srl_ddpg_act``: the clipped noisy action of an env batch, ``mode`` 0 no noise, 1 normal, 2 Ornstein-Uhlenbeck.  Owns the sampling
     record ``rng`` and the per-env OU state ``ou`` (float32 [n, A], from 0)."""
+    _arena_floats = "srl_ddpg_arena_floats"
     NONE, NORMAL, OU = 0, 1, 2
 
     def __init__(self, library, nets, n, seed, sigma, theta=0.15, dt=1e-2, env_offset=0):
@@ -589,9 +588,10 @@ class FusedDDPGAct(_FusedDDPG):
         self._check(rc, "srl_ddpg_act")
 
 
-class FusedDDPGPrepare(_FusedDDPG):
+class FusedDDPGPrepare(_FusedArena):
     """``srl_ddpg_prepare``: sample indices, the critic targets ``y``, ``mu`` and the actor's head derivatives ``d_actor`` of ``batch`` samples
     of the ring (``FusedSACStore``'s).  Owns the sampling record ``rng`` and the outputs."""
+    _arena_floats = "srl_ddpg_arena_floats"
 
     def __init__(self, library, nets, ring, batch, seed):
         import torch
@@ -611,9 +611,10 @@ class FusedDDPGPrepare(_FusedDDPG):
         self._check(rc, "srl_ddpg_prepare")
 
 
-class FusedDDPGGrad(_FusedDDPG):
+class FusedDDPGGrad(_FusedArena):
     """``srl_ddpg_grad``: the weight gradients of the actor and the L2-regularised critic into the gradient arena ``grad`` from what
     :class:`FusedDDPGPrepare` left.  Owns its workspace."""
+    _arena_floats = "srl_ddpg_arena_floats"
 
     def __init__(self, library, nets, batch, critic_l2_reg):
         import torch
@@ -631,9 +632,10 @@ class FusedDDPGGrad(_FusedDDPG):
         self._check(rc, "srl_ddpg_grad")
 
 
-class FusedDDPGAdam(_FusedDDPG):
+class FusedDDPGAdam(_FusedArena):
     """``srl_ddpg_adam``: MpiAdam over the whole arena and the Polyak update of both targets in one launch.  Owns the slots ``m``, ``v``, the
     step count ``t`` (int64 [1]) and the learning rates ``lr`` (float64 [2]: actor, critic)."""
+    _arena_floats = "srl_ddpg_arena_floats"
 
     def __init__(self, library, nets, actor_lr, critic_lr, tau, beta1=0.9, beta2=0.999, epsilon=1e-8):
         import torch

@@ -21,7 +21,8 @@ from sac_timing import ClockSampler, card, event_ms  # noqa: E402
 
 
 def kernels(reps):
-    from rl_baselines.ddpg import DDPGNets, ring_bytes
+    from rl_baselines.ddpg import DDPGNets
+    from rl_baselines.offpolicy import ring_bytes
     from srl_sim._abi import load_cuda_library
     from srl_sim.policy import FusedDDPGAct, FusedDDPGAdam, FusedDDPGGrad, FusedDDPGPrepare, FusedSACStore
     lib = load_cuda_library()

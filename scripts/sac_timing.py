@@ -68,7 +68,8 @@ def event_ms(fn, reps, flush):
 
 
 def kernels(reps):
-    from rl_baselines.sac import SACNets, adam_polyak, ring_bytes, sac_losses
+    from rl_baselines.offpolicy import ring_bytes
+    from rl_baselines.sac import SACNets, adam_polyak, sac_losses
     from srl_sim._abi import load_cuda_library
     from srl_sim.policy import FusedSACAct, FusedSACAdam, FusedSACGrad, FusedSACPrepare, FusedSACStore
     lib = load_cuda_library()

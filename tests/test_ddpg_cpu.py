@@ -111,6 +111,11 @@ def test_cadence():
     assert [t for t in range(450) if cadence(t, hp)] == [99, 199, 299, 399] and cadence(99, hp) == 100
     hp.update(nb_rollout_steps=3, nb_train_steps=5)
     assert [(t, cadence(t, hp)) for t in range(10) if cadence(t, hp)] == [(2, 5), (5, 5), (8, 5)]
+    # the blocks of rl_baselines.offpolicy.learn (G = R, or 2 R for an odd R when captured) start at multiples of G: every full block has
+    # one pattern of gradient steps, so the shared graph rule replays every full block after the first gradient step
+    for R, G in ((3, 6), (3, 3), (4, 4), (100, 100)):
+        hp.update(nb_rollout_steps=R)
+        assert len({tuple(cadence(t, hp) for t in range(t0, t0 + G)) for t0 in range(0, 30 * G, G)}) == 1
 
 
 @pytest.mark.parametrize("noise", ["ou", "normal", "none"])
