@@ -27,6 +27,10 @@
  *                   <- stable-baselines 2.5 `DDPG.learn` with its `MlpPolicy` (chosen by rl_baselines/rl_algorithm/ddpg.py): `_policy` with
  *                      its action noise, `Memory.append` / `sample`, the losses and gradients of `_train_step`, its two `MpiAdam`s and
  *                      `_update_target_net`
+ *   srl_trpo_surrogate, srl_trpo_fvp, srl_trpo_trial, srl_trpo_vector, srl_trpo_vf_grad, srl_trpo_vf_adam
+ *                   <- stable-baselines 2.5 `TRPO.learn` with `MlpPolicy` (chosen by rl_baselines/rl_algorithm/trpo.py): `compute_lossandgrad`,
+ *                      `compute_fvp` (+ cg_damping), baselines' `cg`, the step size and backtracking line search over `compute_losses`,
+ *                      and the value function's `compute_vflossandgrad` with its `MpiAdam`
  *
  * Conventions are those of srl_sim.h: 0 on success, message from srl_sim_last_error(); all pointers are DEVICE pointers;
  * calls are asynchronous on `stream` and capturable into a CUDA graph (everything a launch reads that changes between
@@ -357,6 +361,78 @@ int srl_ddpg_grad(const srl_ddpg_nets* nets, const float* obs_ring, const float*
  *   step : i64[1], the optimiser steps taken;  lr : f64[2] {actor_lr, critic_lr} */
 int srl_ddpg_adam(const srl_ddpg_nets* nets, const float* grad, float* m, float* v, int64_t* step, const double* lr, double beta1, double beta2,
                   double epsilon, double tau, void* stream);
+
+/* ---- TRPO (rl_baselines/trpo.py) ----
+ * stable-baselines 2.5 `TRPO` with `MlpPolicy` (chosen by rl_baselines/rl_algorithm/trpo.py): the policy is an srl_mlp_policy (tanh towers).
+ * RECALLED from stable-baselines 2.5 / baselines' trpo_mpi, not checked against an installed copy (none can be installed here): the losses
+ * (ratio against a copy of the policy, surrgain, meankl, meanent, optimgain = surrgain + entcoeff meanent), the population-std advantage
+ * standardisation without epsilon, the Fisher-vector product on every 5th sample plus cg_damping v, baselines' cg() with residual_tol 1e-10,
+ * lm = sqrt(|shs| / max_kl), the ten-trial backtracking line search (reject non-finite losses, meankl > 1.5 max_kl or a negative improvement;
+ * restore theta_old after ten rejections), the np.allclose(g, 0) skip, and the value function's MpiAdam on mean((v - ret)^2) (no 1/2).
+ * The FLAT vector of the policy tower is pi_w1, pi_b1, pi_w2, pi_b2, pi_w3, pi_b3, logstd (Box only), each in torch layout; the value tower's
+ * is vf_w1 .. vf_b3.  Products are the Gauss-Newton form of the KL's Hessian at theta_old (equal to TF's double backprop there): Categorical
+ * J^T (diag(p) - p p^T) J v, DiagGaussian J^T diag(1 / sigma^2) J v on the mean head and 2 v on logstd, all over the mean of the rows.
+ * Every launch is asynchronous on `stream`, capturable, and deterministic (per-CTA partials summed in float64 in CTA order). */
+size_t srl_trpo_flat_floats(int obs_dim, int n_out, int discrete);     /* the flat pi vector's length P; 0 for an unsupported shape */
+/* workspace of every chunked entry point below over `rows` rows (no state between calls) */
+size_t srl_trpo_workspace_bytes(int obs_dim, int n_out, int rows);
+
+/* At theta_old over rows 0 .. rows - 1: atarg = (adv - mean) / std (population std, no epsilon; float32 result written per row), the old head
+ * outputs old_out f32[rows, n_out] (logits / means), the gradient of optimgain (ratio = 1) into grad f32[P] and losses f64[3] = {surrgain,
+ * meankl (0), meanent}.  actions: i64[rows] (Discrete) / f32[rows, n_out] (Box, the unclipped samples). */
+int srl_trpo_surrogate(const srl_mlp_policy* policy, int rows, const float* obs, const void* actions, const float* adv, float ent_coef, float* atarg,
+                       float* old_out, float* grad, double* losses, void* workspace, size_t workspace_bytes, void* stream);
+
+/* out = F v + damping v, F the mean Fisher matrix of the pi tower at the policy's weights over `rows` samples: sample s is row
+ * (s / group) group_stride + s % group of obs (TRPO's every-5th-step subsample of a [T, N] rollout: group = N, group_stride = 5 N).
+ * v, out : f32[P] flat vectors (they must not alias). */
+int srl_trpo_fvp(const srl_mlp_policy* policy, int rows, int group, int group_stride, const float* obs, const float* v, float damping, float* out,
+                 void* workspace, size_t workspace_bytes, void* stream);
+
+/* The losses of one line-search trial at theta = theta_old + s fullstep, s = state[SRL_TRPO_SCALE] (float32: w + fullstep s, the value the
+ * update writes), against the old outputs and atarg srl_trpo_surrogate left: losses f64[3] = {mean(ratio atarg), mean KL(old || new),
+ * mean entropy}.  Does nothing once the status record says the trial need not run (skipped, non-finite step, accepted, ten trials). */
+int srl_trpo_trial(const srl_mlp_policy* policy, int rows, const float* obs, const void* actions, const float* atarg, const float* old_out,
+                   const float* fullstep, const double* state, double* losses, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The gradient of mean((v - ret[g])^2) over the rows g = idx[0 .. rows - 1] (idx NULL: rows 0 .. rows - 1) into grad f32[value P]. */
+int srl_trpo_vf_grad(const srl_mlp_policy* policy, int rows, const int64_t* idx, const float* obs, const float* ret, float* grad, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
+/* The status record state f64[SRL_TRPO_STATE_DOUBLES] of one update (written by srl_trpo_vector, read by srl_trpo_trial and the host) */
+#define SRL_TRPO_SKIP          0   /* 1: np.allclose(g, 0), the policy is not updated                                      */
+#define SRL_TRPO_CG_ITERS      1   /* CG iterations run                                                                    */
+#define SRL_TRPO_CG_DONE       2   /* 1: r.r < residual_tol was reached; later iterations are no-ops                       */
+#define SRL_TRPO_NONFINITE     3   /* 1: stepdir has a non-finite entry (the reference asserts); no trial runs             */
+#define SRL_TRPO_ACCEPTED      4   /* index of the accepted trial, -1 while none is                                        */
+#define SRL_TRPO_RESTORED      5   /* 1: all ten trials were rejected and theta_old stays                                  */
+#define SRL_TRPO_SCALE         6   /* the step fraction of the next trial: 1, 1/2, 1/4, ...                                */
+#define SRL_TRPO_TRIALS        7   /* trials decided                                                                      */
+#define SRL_TRPO_RDOTR         8   /* r.r of the CG state                                                                 */
+#define SRL_TRPO_GAIN_BEFORE   9   /* optimgain at theta_old                                                              */
+#define SRL_TRPO_SURR_BEFORE  10
+#define SRL_TRPO_ENT_BEFORE   11
+#define SRL_TRPO_SHS          12   /* 0.5 stepdir . F stepdir                                                             */
+#define SRL_TRPO_LM           13   /* sqrt(|shs| / max_kl)                                                                */
+#define SRL_TRPO_TRIAL_LOSSES 16   /* 10 x {optimgain, meankl, meanent} of the trials decided                             */
+#define SRL_TRPO_MAX_TRIALS   10
+#define SRL_TRPO_STATE_DOUBLES 48
+#define SRL_TRPO_OP_START 0        /* after srl_trpo_surrogate: reset the record, the zero-gradient check, x = 0, r = p = g   */
+#define SRL_TRPO_OP_CG    1        /* after z = F p: one iteration of baselines' cg()                                        */
+#define SRL_TRPO_OP_STEP  2        /* after z = F x: shs, lm, fullstep = x / lm, the non-finite stepdir flag                 */
+#define SRL_TRPO_OP_TRIAL 3        /* after srl_trpo_trial: accept (params += s fullstep) or halve s; restore after ten       */
+/* One CTA over the flat vectors vecs f32[6][P] = {g, x, r, p, z, fullstep}: g is srl_trpo_surrogate's gradient, z the last product; the fvp input
+ * is p during CG and x for the step.  Dot products in float64 in a fixed order, vectors in float32.  losses: the f64[3] of the last
+ * srl_trpo_surrogate (START) or srl_trpo_trial (TRIAL).  params (TRIAL): the policy's tensors in srl_mlp_grads layout, updated in place
+ * only on acceptance. */
+int srl_trpo_vector(int op, int obs_dim, int n_out, int discrete, const srl_mlp_grads* params, float* vecs, double* state, const double* losses,
+                    float max_kl, float ent_coef, float residual_tol, void* stream);
+
+/* MpiAdam over the value tower (srl_ddpg_adam's statement with one learning rate and no target): t = *step + 1 (written back),
+ * a = lr sqrt(1 - beta2^t) / (1 - beta1^t) in float64, then in float32 m = beta1 m + (1 - beta1) g; v = beta2 v + (1 - beta2) g^2;
+ * w += ((-a) m) / (sqrt(v) + epsilon).  params: vf_* pointers used; grad, m, v f32[value P]. */
+int srl_trpo_vf_adam(int obs_dim, const srl_mlp_grads* params, const float* grad, float* m, float* v, int64_t* step, double lr, double beta1,
+                     double beta2, double epsilon, void* stream);
 
 #ifdef __cplusplus
 }

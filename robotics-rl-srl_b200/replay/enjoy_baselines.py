@@ -43,7 +43,7 @@ def loadConfigAndSetup(load_args):
     with open(os.path.join(log_dir, "args.json")) as f:
         train_args = json.load(f)
     algo = train_args.get("algo", "ppo2")
-    if algo not in ("ppo2", "a2c", "deepq", "sac", "ddpg"):
+    if algo not in ("ppo2", "a2c", "trpo", "deepq", "sac", "ddpg"):
         raise ValueError(algo + " is not supported for replay")
     env_kwargs = dict(env_globals)
     env_kwargs["shape_reward"] = load_args.shape_reward            # reward sparse or shaped: chosen at replay time (:88)

@@ -1,7 +1,7 @@
 """
 Mirror of the reference's training entry point ``python -m rl_baselines.train`` (rl_baselines/train.py:172-333) for the
 algorithms this repo provides as consumers of the simulator: ``ppo2`` (rl_baselines/ppo2.py), ``a2c`` (rl_baselines/a2c.py), ``deepq``
-(rl_baselines/deepq.py), ``sac`` (rl_baselines/sac.py), ``ddpg`` (rl_baselines/ddpg.py) and ``random_agent`` (rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the
+(rl_baselines/deepq.py), ``sac`` (rl_baselines/sac.py), ``ddpg`` (rl_baselines/ddpg.py), ``trpo`` (rl_baselines/trpo.py) and ``random_agent`` (rl_baselines/random_agent.py:28-42).  Same flag names; ``--num-cpu`` is the number of envs in the
 batch (per GPU when launched with ``torchrun --nproc-per-node N -m rl_baselines.train``: data-parallel PPO2, A2C or DQN, see rl_baselines/ppo2.py).
 """
 import argparse
@@ -24,7 +24,11 @@ SAC_OPT_PARAM = {"ent_coef": float, "learning_rate": float, "gradient_steps": in
 # rl_baselines/rl_algorithm/ddpg.py (DDPGModel.getOptParam)
 DDPG_OPT_PARAM = {"reward_scale": float, "critic_l2_reg": float, "actor_lr": float, "critic_lr": float, "gamma": float, "nb_train_steps": int,
                   "nb_rollout_steps": int, "nb_eval_steps": int, "batch_size": int, "tau": float, "noise_action_sigma": float, "noise_action": str}
-OPT_PARAM = {"ppo2": PPO2_OPT_PARAM, "a2c": A2C_OPT_PARAM, "deepq": DQN_OPT_PARAM, "sac": SAC_OPT_PARAM, "ddpg": DDPG_OPT_PARAM}
+# rl_baselines/rl_algorithm/trpo.py (TRPOModel.getOptParam)
+TRPO_OPT_PARAM = {"timesteps_per_batch": int, "max_kl": float, "cg_iters": int, "gamma": float, "lam": float, "entcoeff": float,
+                  "cg_damping": float, "vf_stepsize": float, "vf_iters": int}
+OPT_PARAM = {"ppo2": PPO2_OPT_PARAM, "a2c": A2C_OPT_PARAM, "deepq": DQN_OPT_PARAM, "sac": SAC_OPT_PARAM, "ddpg": DDPG_OPT_PARAM,
+             "trpo": TRPO_OPT_PARAM}
 LR_SCHEDULES = ['linear', 'constant', 'double_linear_con', 'middle_drop', 'double_middle_drop']
 
 
@@ -43,13 +47,13 @@ def parserHyperParam(pairs, opt_param=PPO2_OPT_PARAM):
 
 def main(argv=None):
     parser = argparse.ArgumentParser(description="Train script for RL algorithms")
-    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'a2c', 'deepq', 'sac', 'ddpg', 'random_agent'], type=str)
+    parser.add_argument('--algo', default='ppo2', choices=['ppo2', 'a2c', 'deepq', 'sac', 'ddpg', 'trpo', 'random_agent'], type=str)
     parser.add_argument('--env', type=str, help='environment ID', default='KukaButtonGymEnv-v0', choices=list(registered_env.keys()))
     parser.add_argument('--seed', type=int, default=0)
     parser.add_argument('--episode_window', type=int, default=40, help='Episode window for moving average plot (default: 40)')
     parser.add_argument('--num-stack', type=int, default=1, help='number of frames to stack (default: 1)')
     parser.add_argument('-joints', '--action-joints', action='store_true', default=False, help='set actions to the joints of the arm directly')
-    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 / A2C / DQN / SAC / DDPG hyper-parameters as name:value pairs')
+    parser.add_argument('--hyperparam', type=str, nargs='+', default=[], help='PPO2 / A2C / DQN / SAC / DDPG / TRPO hyper-parameters as name:value pairs')
     parser.add_argument('--lr-schedule', help='Learning rate schedule (a2c)', default='constant', choices=LR_SCHEDULES)
     parser.add_argument('--log-dir', default='/tmp/gym/', type=str)
     parser.add_argument('--num-timesteps', type=int, default=int(1e6))
@@ -107,7 +111,7 @@ def main(argv=None):
         env_kwargs["action_joints"] = True
     log_dir = os.path.join(args.log_dir, args.env, args.srl_model, args.algo, time.strftime("%y-%m-%d_%Hh%M_%S"))
     num_timesteps = int(1.1 * args.num_timesteps)      # the reference trains 10 % longer (train.py:319)
-    if args.algo in ("ppo2", "a2c", "deepq", "sac", "ddpg"):
+    if args.algo in ("ppo2", "a2c", "deepq", "sac", "ddpg", "trpo"):
         if args.algo == "ppo2":
             from rl_baselines.ppo2 import train
         elif args.algo == "a2c":
@@ -116,6 +120,8 @@ def main(argv=None):
             from rl_baselines.sac import train
         elif args.algo == "ddpg":
             from rl_baselines.ddpg import train
+        elif args.algo == "trpo":
+            from rl_baselines.trpo import train
         else:
             from rl_baselines.deepq import train
         from srl_sim.distributed import rank_world

@@ -16,7 +16,8 @@ POLICY_EXPORTS = ["srl_policy_act", "srl_obs_filter", "srl_obs_stack_filter", "s
                   "srl_a2c_grad", "srl_a2c_workspace_bytes", "srl_clip_rmsprop", "srl_dqn_act", "srl_dqn_target", "srl_dqn_grad", "srl_clip_adam",
                   "srl_replay_add", "srl_replay_sample", "srl_replay_update", "srl_sac_arena_floats", "srl_sac_workspace_bytes", "srl_sac_act",
                   "srl_sac_store", "srl_sac_prepare", "srl_sac_grad", "srl_sac_adam", "srl_ddpg_arena_floats", "srl_ddpg_workspace_bytes",
-                  "srl_ddpg_act", "srl_ddpg_prepare", "srl_ddpg_grad", "srl_ddpg_adam"]
+                  "srl_ddpg_act", "srl_ddpg_prepare", "srl_ddpg_grad", "srl_ddpg_adam", "srl_trpo_flat_floats", "srl_trpo_workspace_bytes",
+                  "srl_trpo_surrogate", "srl_trpo_fvp", "srl_trpo_trial", "srl_trpo_vf_grad", "srl_trpo_vector", "srl_trpo_vf_adam"]
 GRAD_NAMES = ["pi_w1", "pi_b1", "pi_w2", "pi_b2", "pi_w3", "pi_b3", "vf_w1", "vf_b1", "vf_w2", "vf_b2", "vf_w3", "vf_b3", "logstd"]
 
 
@@ -112,6 +113,22 @@ def bind(cdll):
     cdll.srl_ddpg_grad.argtypes = [S, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_size_t, c_void_p]
     cdll.srl_ddpg_adam.restype = c_int
     cdll.srl_ddpg_adam.argtypes = [S, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_double, c_void_p]
+    cdll.srl_trpo_flat_floats.restype = c_size_t
+    cdll.srl_trpo_flat_floats.argtypes = [c_int, c_int, c_int]
+    cdll.srl_trpo_workspace_bytes.restype = c_size_t
+    cdll.srl_trpo_workspace_bytes.argtypes = [c_int, c_int, c_int]
+    cdll.srl_trpo_surrogate.restype = c_int
+    cdll.srl_trpo_surrogate.argtypes = [P, c_int, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_trpo_fvp.restype = c_int
+    cdll.srl_trpo_fvp.argtypes = [P, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_trpo_trial.restype = c_int
+    cdll.srl_trpo_trial.argtypes = [P, c_int] + [c_void_p] * 7 + [c_void_p, c_size_t, c_void_p]
+    cdll.srl_trpo_vf_grad.restype = c_int
+    cdll.srl_trpo_vf_grad.argtypes = [P, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]
+    cdll.srl_trpo_vector.restype = c_int
+    cdll.srl_trpo_vector.argtypes = [c_int, c_int, c_int, c_int, G, c_void_p, c_void_p, c_void_p, c_float, c_float, c_float, c_void_p]
+    cdll.srl_trpo_vf_adam.restype = c_int
+    cdll.srl_trpo_vf_adam.argtypes = [c_int, G, c_void_p, c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_double, c_void_p]
     return cdll
 
 
@@ -154,6 +171,15 @@ def policy_struct(policy):
         setattr(s, name, t.data_ptr())
     s.logstd = None if policy.discrete else policy.logstd.data_ptr()
     return s, tensors
+
+
+def ppo2_gae(library, rew, value, done, last_value, gamma, lam, adv_out, ret_out, stream=None):
+    """``srl_ppo2_gae`` on the loaded CUDA library: GAE(lambda) of a [T, N] rollout in one launch (float32 tensors; ``done`` holds 1.0 where an
+    episode ended)."""
+    T, N = rew.shape
+    rc = bind(library.lib).srl_ppo2_gae(int(T), int(N), rew.data_ptr(), value.data_ptr(), done.data_ptr(), last_value.data_ptr(), float(gamma),
+                                        float(lam), adv_out.data_ptr(), ret_out.data_ptr(), stream)
+    library.check(rc, "srl_ppo2_gae")
 
 
 class FusedObsFilter(object):
@@ -248,10 +274,7 @@ class FusedPPO2Grad(object):
 
     def gae(self, rew, value, done, last_value, gamma, lam, adv_out, ret_out, stream=None):
         """``srl_ppo2_gae``: GAE(lambda) of a [T, N] rollout in one launch (float32 tensors; ``done`` holds 1.0 where an episode ended)."""
-        T, N = rew.shape
-        rc = self._lib.srl_ppo2_gae(int(T), int(N), rew.data_ptr(), value.data_ptr(), done.data_ptr(), last_value.data_ptr(), float(gamma), float(lam),
-                                    adv_out.data_ptr(), ret_out.data_ptr(), stream)
-        self._library.check(rc, "srl_ppo2_gae")
+        ppo2_gae(self._library, rew, value, done, last_value, gamma, lam, adv_out, ret_out, stream)
 
     def __call__(self, idx, obs, actions, adv, ret, old_logp, old_value, cliprange, ent_coef, vf_coef, stream=None):
         """All arguments are CUDA tensors of the whole rollout (``idx``: int64 [minibatch] rows, or None for the first ``minibatch`` rows)."""
@@ -649,3 +672,84 @@ class FusedDDPGAdam(_FusedArena):
         rc = self._lib.srl_ddpg_adam(byref(self.struct), grad.data_ptr(), self.m.data_ptr(), self.v.data_ptr(), self.t.data_ptr(), self.lr.data_ptr(),
                                      self.beta1, self.beta2, self.epsilon, self.tau, stream)
         self._check(rc, "srl_ddpg_adam")
+
+
+# ---- TRPO (include/srl_policy.h: srl_trpo_*; rl_baselines/trpo.py) ----
+
+# the status record's slots (include/srl_policy.h: SRL_TRPO_*)
+TRPO_SKIP, TRPO_CG_ITERS, TRPO_CG_DONE, TRPO_NONFINITE, TRPO_ACCEPTED, TRPO_RESTORED, TRPO_SCALE, TRPO_TRIALS = range(8)
+TRPO_RDOTR, TRPO_GAIN_BEFORE, TRPO_SURR_BEFORE, TRPO_ENT_BEFORE, TRPO_SHS, TRPO_LM = range(8, 14)
+TRPO_TRIAL_LOSSES, TRPO_MAX_TRIALS, TRPO_STATE_DOUBLES = 16, 10, 48
+TRPO_OP_START, TRPO_OP_CG, TRPO_OP_STEP, TRPO_OP_TRIAL = range(4)
+
+
+class FusedTRPO(object):
+    """TRPO's update on the CUDA library for one ``MlpPolicy`` and a rollout of ``rows`` rows: the chunked tower kernel in its four modes
+    (``surrogate``, ``fvp``, ``trial``, ``vf_grad``), the single-CTA ``vector`` kernel that holds the CG state, the step and the line-search
+    decision, and the value tower's MpiAdam (``vf_adam``).  Owns every device buffer the update needs:
+      ``atarg`` f32[rows], ``old_out`` f32[rows, n_out], ``vecs`` f32[6, P] = {g, x, r, p, z, fullstep} over the flat pi vector,
+      ``state`` f64[48] the status record, ``losses`` f64[3], ``vgrad`` f32[value P] and the value optimiser's ``m``, ``v``, ``step``."""
+
+    def __init__(self, library, policy, rows):
+        import torch
+        self._lib = bind(library.lib)
+        self._library = library
+        self.struct, self._keep = policy_struct(policy)
+        dev = policy.pi[0].weight.device
+        if dev.type != "cuda":
+            raise ValueError("FusedTRPO needs a policy on a CUDA device (there is no CPU fallback)")
+        self.params = policy_params(policy)
+        self._p = tensors_struct(self.params)
+        D, A, disc = self.struct.obs_dim, self.struct.n_out, self.struct.discrete
+        self.P = int(self._lib.srl_trpo_flat_floats(D, A, disc))
+        self.Pv = int(self._lib.srl_trpo_flat_floats(D, 1, 1))
+        self.rows = int(rows)
+        nbytes = int(self._lib.srl_trpo_workspace_bytes(D, A, self.rows))
+        if self.P <= 0 or nbytes <= 0:
+            raise ValueError("srl_trpo_workspace_bytes: unsupported shape")
+        self.workspace = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
+        z = lambda *shape, dtype=torch.float32: torch.zeros(shape, dtype=dtype, device=dev)
+        self.atarg, self.old_out, self.vecs = z(self.rows), z(self.rows, A), z(6, self.P)
+        self.g, self.x, self.r, self.p, self.z, self.fullstep = self.vecs.unbind(0)
+        self.state, self.losses = z(TRPO_STATE_DOUBLES, dtype=torch.float64), z(3, dtype=torch.float64)
+        self.vgrad, self.m, self.v = z(self.Pv), z(self.Pv), z(self.Pv)
+        self.step = z(1, dtype=torch.int64)
+
+    def _check(self, rc, name):
+        self._library.check(rc, name)
+
+    def surrogate(self, obs, actions, adv, ent_coef, stream=None):
+        """At theta_old over all rows: ``atarg``, ``old_out``, the gradient of optimgain into ``g`` and the losses before the step."""
+        rc = self._lib.srl_trpo_surrogate(byref(self.struct), self.rows, obs.data_ptr(), actions.data_ptr(), adv.data_ptr(), float(ent_coef),
+                                          self.atarg.data_ptr(), self.old_out.data_ptr(), self.g.data_ptr(), self.losses.data_ptr(),
+                                          self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._check(rc, "srl_trpo_surrogate")
+
+    def fvp(self, rows, group, group_stride, obs, v, damping, out, stream=None):
+        """out = F v + damping v over ``rows`` samples, sample s at row (s // group) group_stride + s % group of ``obs``."""
+        rc = self._lib.srl_trpo_fvp(byref(self.struct), int(rows), int(group), int(group_stride), obs.data_ptr(), v.data_ptr(), float(damping),
+                                    out.data_ptr(), self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._check(rc, "srl_trpo_fvp")
+
+    def trial(self, obs, actions, stream=None):
+        """The losses of the trial at theta_old + state[SCALE] fullstep into ``losses`` (no-op once the record says no trial runs)."""
+        rc = self._lib.srl_trpo_trial(byref(self.struct), self.rows, obs.data_ptr(), actions.data_ptr(), self.atarg.data_ptr(), self.old_out.data_ptr(),
+                                      self.fullstep.data_ptr(), self.state.data_ptr(), self.losses.data_ptr(), self.workspace.data_ptr(),
+                                      self.workspace.numel(), stream)
+        self._check(rc, "srl_trpo_trial")
+
+    def vector(self, op, max_kl, ent_coef, residual_tol=1e-10, stream=None):
+        rc = self._lib.srl_trpo_vector(int(op), self.struct.obs_dim, self.struct.n_out, self.struct.discrete, byref(self._p), self.vecs.data_ptr(),
+                                       self.state.data_ptr(), self.losses.data_ptr(), float(max_kl), float(ent_coef), float(residual_tol), stream)
+        self._check(rc, "srl_trpo_vector")
+
+    def vf_grad(self, rows, idx, obs, ret, stream=None):
+        """The gradient of mean((v - ret)^2) over ``rows`` rows ``idx`` (None: the first rows) into ``vgrad``."""
+        rc = self._lib.srl_trpo_vf_grad(byref(self.struct), int(rows), None if idx is None else idx.data_ptr(), obs.data_ptr(), ret.data_ptr(),
+                                        self.vgrad.data_ptr(), self.workspace.data_ptr(), self.workspace.numel(), stream)
+        self._check(rc, "srl_trpo_vf_grad")
+
+    def vf_adam(self, lr, beta1=0.9, beta2=0.999, epsilon=1e-8, stream=None):
+        rc = self._lib.srl_trpo_vf_adam(self.struct.obs_dim, byref(self._p), self.vgrad.data_ptr(), self.m.data_ptr(), self.v.data_ptr(),
+                                        self.step.data_ptr(), float(lr), float(beta1), float(beta2), float(epsilon), stream)
+        self._check(rc, "srl_trpo_vf_adam")
