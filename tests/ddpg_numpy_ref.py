@@ -112,13 +112,15 @@ def ou_model(state, z, prev_done, sigma, theta=0.15, dt=1e-2):
     return x + theta * (0.0 - x) * dt + sigma * math.sqrt(dt) * np.asarray(z, np.float64)
 
 
-def mpi_adam_polyak_f32(arena, target, grads, actor_end, actor_lr, critic_lr, tau, beta1=0.9, beta2=0.999, eps=1e-8):
+def mpi_adam_polyak_f32(arena, target, grads, actor_end, actor_lr, critic_lr, tau, beta1=0.9, beta2=0.999, eps=1e-8, m=None, v=None, steps=0):
     """MpiAdam.update (a in float64, then every array operation in float32, python floats rounded to float32 as numpy 1.x does) for each
-    gradient, each step followed by the Polyak update of the targets.  Returns (arena, target, m, v)."""
+    gradient, each step followed by the Polyak update of the targets.  The slots ``m``, ``v`` (default 0) are those left by ``steps``
+    earlier updates, so the first update here has MpiAdam's t = steps + 1.  Returns (arena, target, m, v)."""
     f32 = np.float32
     w, tg = np.array(arena, f32), np.array(target, f32)
-    m, v = np.zeros_like(w), np.zeros_like(w)
-    for t, g in enumerate(grads, 1):
+    m = np.zeros_like(w) if m is None else np.array(m, f32)
+    v = np.zeros_like(w) if v is None else np.array(v, f32)
+    for t, g in enumerate(grads, int(steps) + 1):
         g = np.asarray(g, f32)
         neg_a = np.empty_like(w)
         for lo, hi, lr in ((0, actor_end, actor_lr), (actor_end, w.size, critic_lr)):

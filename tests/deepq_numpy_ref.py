@@ -7,7 +7,8 @@ srl_clip_adam) and not from rl_baselines/deepq.py, for the CPU and GPU tests of 
   clip_adam_model     : tf.clip_by_norm per tensor followed by TF1 Adam, on lists of arrays
   SegmentTree / PrioritizedReplay : a direct transcription of baselines' SegmentTree (loop form) and of the prioritized buffer's bookkeeping
   first_sample_model  : the indices of a replay's first batch, while every stored leaf is still 1^alpha (uniform or prioritized)
-  dqn_step_model      : one gradient step from zero Adam slots (double Q with one network as online and target, gradient, clip, Adam)
+  tree_sample_model   : the indices and importance weights of a batch drawn from any sum / min trees (find_prefixsum_idx, vectorised)
+  dqn_step_model      : one gradient step (double Q with its own online and target networks, gradient, clip, Adam from given slots)
 """
 import operator
 
@@ -172,13 +173,36 @@ def first_sample_model(u, n, tree_cap, prioritized, boundary=1e-11):
     return np.minimum(node - tree_cap, n - 1), np.abs(un - np.round(un)) <= boundary * n
 
 
-def dqn_step_model(qnet, obs, act, rew, done, next_obs, gamma, lr, clip_norm, beta1, beta2, eps):
-    """One gradient step of a DQN whose online and target networks are both ``qnet`` and whose Adam slots are zero, over sampled rows with
-    importance weights 1: y (double Q), td and the gradients, the per-tensor clip factors, and the parameters and slots after the step."""
-    y, _ = double_q_model(qnet, qnet, rew, done, next_obs, gamma)
-    grads, td = dqn_grads_model(qnet, obs, act, y, np.ones(len(y)))
+def tree_sample_model(sum_tree, min_tree, size, tree_cap, u, beta, prioritized=True):
+    """PrioritizedReplayBuffer.sample over the float64 trees ``sum_tree`` / ``min_tree`` (root 1, leaf i at tree_cap + i) holding ``size``
+    transitions, for the uniforms ``u``: find_prefixsum_idx at mass u * total, one tree level per pass for every sample at once, a walk into
+    an empty leaf clamped to size - 1, and weights (p_i size)^-beta / (p_min size)^-beta.  Uniform replay: min(floor(u size), size - 1) and
+    weights 1.  Returns (idx, float32 weights)."""
+    u, n = np.asarray(u, np.float64), int(size)
+    if not prioritized:
+        return np.minimum((u * n).astype(np.int64), n - 1), np.ones(len(u), np.float32)
+    s = np.asarray(sum_tree, np.float64)
+    total = s[1]
+    mass, node = u * total, np.ones(len(u), np.int64)
+    while node[0] < tree_cap:
+        left = s[2 * node]
+        right = left <= mass
+        mass = np.where(right, mass - left, mass)
+        node = 2 * node + right
+    idx = np.minimum(node - tree_cap, n - 1)
+    max_weight = (min_tree[1] / total * n) ** (-beta)
+    return idx, ((s[tree_cap + idx] / total * n) ** (-beta) / max_weight).astype(np.float32)
+
+
+def dqn_step_model(qnet, obs, act, rew, done, next_obs, gamma, lr, clip_norm, beta1, beta2, eps, target=None, weights=None, m=None, v=None,
+                   step=1):
+    """One gradient step of a DQN with online network ``qnet`` and target network ``target`` (default: ``qnet`` itself) over sampled rows
+    with importance ``weights`` (default 1), from the Adam slots ``m``, ``v`` (default 0) at TF's step ``step`` (1-based): y (double Q), td
+    and the gradients, the per-tensor clip factors, and the parameters and slots after the step."""
+    y, _ = double_q_model(qnet, qnet if target is None else target, rew, done, next_obs, gamma)
+    grads, td = dqn_grads_model(qnet, obs, act, y, np.ones(len(y)) if weights is None else weights)
     params = [p.detach().cpu().double().numpy() for p in qnet.parameters()]
-    new, m, v = clip_adam_model(params, grads, [np.zeros(p.shape) for p in params], [np.zeros(p.shape) for p in params], 1, lr, clip_norm,
-                                beta1, beta2, eps)
+    zeros = [np.zeros(p.shape) for p in params]
+    new, m, v = clip_adam_model(params, grads, zeros if m is None else m, zeros if v is None else v, step, lr, clip_norm, beta1, beta2, eps)
     scale = [clip_norm / max(np.sqrt((g * g).sum()), clip_norm) for g in grads]
     return dict(y=y, td=td, grads=grads, clip_scale=scale, params=params, new_params=new, m=m, v=v)

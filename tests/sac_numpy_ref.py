@@ -96,14 +96,16 @@ def sac_step_model(arena, target, W, A, obs, act, rew, next_obs, done, eps, gamm
     return grad, dict(q_backup=q_backup, v_backup=v_backup, logp=logp, d_actor=d_actor)
 
 
-def adam_polyak_model(arena, target, grads, W, A, lr, tau, beta1=0.9, beta2=0.999, eps=1e-8):
-    """TF1 Adam (slots from 0, t from 1) over the arena for each gradient in ``grads``, each step followed by target = (1 - tau) target +
-    tau vf.  Float64; returns (arena, target, m, v)."""
+def adam_polyak_model(arena, target, grads, W, A, lr, tau, beta1=0.9, beta2=0.999, eps=1e-8, m=None, v=None, steps=0):
+    """TF1 Adam over the arena for each gradient in ``grads``, each step followed by target = (1 - tau) target + tau vf.  The slots ``m``,
+    ``v`` (default 0) are those left by ``steps`` earlier steps, so the first step here is t = steps + 1.  Float64; returns (arena, target,
+    m, v)."""
     nets, P = layout(W, A)
     w, tg = np.array(arena, np.float64), np.array(target, np.float64)
-    m, v = np.zeros(P), np.zeros(P)
+    m = np.zeros(P) if m is None else np.array(m, np.float64)
+    v = np.zeros(P) if v is None else np.array(v, np.float64)
     lo = nets["vf"][0]
-    for t, g in enumerate(grads, 1):
+    for t, g in enumerate(grads, int(steps) + 1):
         g = np.asarray(g, np.float64)
         lr_t = lr * math.sqrt(1 - beta2 ** t) / (1 - beta1 ** t)
         m = beta1 * m + (1 - beta1) * g

@@ -67,25 +67,43 @@ def test_ddpg_losses_gradient_matches_the_float64_model(W, A):
     assert np.all(diff[~mask] == 0)
 
 
-def test_torch_mpi_adam_polyak_gives_the_bytes_of_the_numpy_float32_statement():
+def _mpi_adam_polyak_against_the_statement(warm):
+    """One case of test_torch_mpi_adam_polyak_gives_the_bytes_of_the_numpy_float32_statement: ``warm`` torch steps before the compared ones."""
     from rl_baselines.ddpg import DDPGNets, mpi_adam_polyak
     W, A = 3, 3
     torch.manual_seed(0)
     nets = DDPGNets(W, A)
     with torch.no_grad():
         nets.target.add_(0.01 * torch.randn_like(nets.target))
-    arena0, target0 = nets.arena.detach().clone().numpy(), nets.target.clone().numpy()
     m, v, t = torch.zeros_like(nets.arena), torch.zeros_like(nets.arena), torch.zeros(1, dtype=torch.int64)
     g = torch.Generator().manual_seed(1)
+    for _ in range(warm):
+        mpi_adam_polyak(nets, torch.randn(nets.arena.numel(), generator=g), m, v, t, 1e-4, 1e-3, 0.001)
+    arena0, target0, m0, v0 = nets.arena.detach().clone().numpy(), nets.target.clone().numpy(), m.clone().numpy(), v.clone().numpy()
+    assert int(t[0]) == warm and (np.abs(m0).max() > 0) == (warm > 0)
     grads = [torch.randn(nets.arena.numel(), generator=g) * (0.1 + k % 7) for k in range(100)]
     for gr in grads:
         mpi_adam_polyak(nets, gr, m, v, t, 1e-4, 1e-3, 0.001)
-    w, tg, mm, vv = mpi_adam_polyak_f32(arena0, target0, [x.numpy() for x in grads], nets.layout["actor"]["end"], 1e-4, 1e-3, 0.001)
+    w, tg, mm, vv = mpi_adam_polyak_f32(arena0, target0, [x.numpy() for x in grads], nets.layout["actor"]["end"], 1e-4, 1e-3, 0.001, m=m0, v=v0,
+                                        steps=warm)
     for got, want in ((nets.arena.detach(), w), (nets.target, tg), (m, mm), (v, vv)):
         assert got.numpy().dtype == want.dtype == np.float32
         assert np.array_equal(got.numpy(), want)
-    assert int(t[0]) == 100
+    assert int(t[0]) == warm + 100
     assert not np.array_equal(w, arena0) and not np.array_equal(tg, target0)
+    if warm:                                                   # the step count is part of the statement: one off gives other bytes
+        w_off, _, _, _ = mpi_adam_polyak_f32(arena0, target0, [grads[0].numpy()], nets.layout["actor"]["end"], 1e-4, 1e-3, 0.001, m=m0, v=v0,
+                                             steps=warm - 1)
+        w1, _, _, _ = mpi_adam_polyak_f32(arena0, target0, [grads[0].numpy()], nets.layout["actor"]["end"], 1e-4, 1e-3, 0.001, m=m0, v=v0,
+                                          steps=warm)
+        assert not np.array_equal(w_off, w1)
+
+
+def test_torch_mpi_adam_polyak_gives_the_bytes_of_the_numpy_float32_statement():
+    """100 updates of the torch statement give the bytes of the numpy float32 transcription, from zero slots and from the slots, target
+    and step count that 37 earlier updates left."""
+    for warm in (0, 37):
+        _mpi_adam_polyak_against_the_statement(warm)
 
 
 def test_ou_step_and_its_reset_match_numpy():

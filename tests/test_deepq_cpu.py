@@ -15,7 +15,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from conftest import ORACLE_LIB, PKG
-from deepq_numpy_ref import PrioritizedReplay, SegmentTree, clip_adam_model, double_q_model, dqn_grads_model
+from deepq_numpy_ref import PrioritizedReplay, SegmentTree, clip_adam_model, double_q_model, dqn_grads_model, tree_sample_model
 from test_consumer_reference_cpu import grad_bound, grad_errors
 from test_ppo2_distributed_cpu import _free_port
 
@@ -93,17 +93,24 @@ def test_double_q_target_and_argmax_ties():
     assert torch.allclose(y, target(torch.zeros(2, 3))[:, 1])
 
 
-@pytest.mark.parametrize("clip", [0.05, 1e3], ids=["clipped", "unclipped"])
-def test_torch_clip_adam_matches_the_float64_tf_model(clip):
+@pytest.mark.parametrize("clip,warm", [(0.05, 0), (1e3, 0), (0.05, 37)], ids=["clipped", "unclipped", "clipped-after_37_steps"])
+def test_torch_clip_adam_matches_the_float64_tf_model(clip, warm):
+    """100 steps of the torch statement against the float64 model, from zero slots or from the slots and beta powers that ``warm`` earlier
+    steps left (the model told only the slots and its 1-based step)."""
     from rl_baselines.deepq import clip_adam
     q = _qnet(3, 6)
     params = list(q.parameters())
     m, v = [torch.zeros_like(p) for p in params], [torch.zeros_like(p) for p in params]
     bp = torch.tensor([0.9, 0.999])
-    p64 = [p.detach().double().numpy().copy() for p in params]
-    m64, v64 = [np.zeros(p.shape) for p in params], [np.zeros(p.shape) for p in params]
     g = torch.Generator().manual_seed(5)
-    for step in range(1, 101):
+    for _ in range(warm):
+        for p in params:
+            p.grad = torch.randn(p.shape, generator=g) * 0.05
+        clip_adam(params, m, v, bp, 1e-3, clip, 0.9, 0.999, 1e-8)
+    p64 = [p.detach().double().numpy().copy() for p in params]
+    m64, v64 = [mm.double().numpy().copy() for mm in m], [vv.double().numpy().copy() for vv in v]
+    assert (max(np.abs(x).max() for x in m64) > 0) == (warm > 0)
+    for step in range(warm + 1, warm + 101):
         for p in params:
             p.grad = torch.randn(p.shape, generator=g) * 0.05
         assert (max(float(torch.sqrt((p.grad.double() ** 2).sum())) for p in params) > clip) == (clip == 0.05)
@@ -114,30 +121,39 @@ def test_torch_clip_adam_matches_the_float64_tf_model(clip):
         assert np.abs(p.detach().double().numpy() - w).max() <= 1e-3 * 100 * 2e-5 + 100 * 2.0 ** -23 * (np.abs(w).max() + 1.0)
     for mm, w in zip(m, m64):
         assert np.abs(mm.double().numpy() - w).max() <= 1e-5 * (np.abs(w).max() + 1e-6)
-    assert abs(float(bp[0]) - 0.9 ** 101) < 1e-6
+    assert abs(float(bp[0]) - 0.9 ** (warm + 101)) < 1e-6
 
 
 def test_replay_tree_matches_the_segment_tree_transcription():
-    """rl_baselines.deepq.ReplayTree against baselines' SegmentTree loop form: inserts that wrap the ring, duplicates (last wins), max_priority,
-    weights, find_prefixsum_idx on masses at and next to node boundaries, and the clamp of a walk into an empty leaf."""
+    """rl_baselines.deepq.ReplayTree against baselines' SegmentTree loop form: inserts that wrap the ring (13 and 40 of them over 5 rows),
+    duplicates (last wins), max_priority, weights, find_prefixsum_idx on masses at and next to node boundaries, and the clamp of a walk into
+    an empty leaf.  Both, and tree_sample_model on the loop form's trees, sample alike from trees whose leaves hold earlier priorities; a row
+    overwritten after the ring wraps goes back to max_priority^alpha."""
     from rl_baselines.deepq import ReplayTree
-    rows, N = 5, 7
-    vec, loop = ReplayTree(rows, N, 0.6), PrioritizedReplay(rows, N, 0.6)
-    rng = np.random.RandomState(0)
-    for step in range(13):
-        vec.add(step % rows); loop.add_row(step % rows)
-        if step >= 1:
-            u = rng.rand(40)
-            i1, w1 = vec.sample(u, 0.5)
-            i2, w2 = loop.sample(u, 0.5)
-            assert np.array_equal(i1, i2) and np.array_equal(w1, w2)
-            td = rng.randn(40).astype(np.float32) * 3
-            i1[5:9] = i1[0]                              # a repeated index: the last occurrence's priority stays
-            vec.update(i1, td, 1e-6); loop.update_priorities(i1, td, 1e-6)
-            assert vec.sum[vec.tree_cap + i1[0]] == float(np.float32(abs(td[8])) + np.float32(1e-6)) ** 0.6 or i1[0] in i1[9:]
-        s, m = loop.trees()
-        assert np.array_equal(vec.sum[1:], s[1:]) and np.array_equal(vec.min[1:], m[1:]) and vec.max_priority == loop.max_priority
-        assert vec.size == loop.size == min(step + 1, rows) * N
+    for steps in (13, 40):
+        rows, N = 5, 7
+        vec, loop = ReplayTree(rows, N, 0.6), PrioritizedReplay(rows, N, 0.6)
+        rng = np.random.RandomState(0)
+        for step in range(steps):
+            vec.add(step % rows); loop.add_row(step % rows)
+            s, m = loop.trees()
+            if step >= rows:                                 # the row just overwritten holds max_priority^alpha again, the others kept theirs
+                leaf = s[loop.tree_cap:loop.tree_cap + rows * N].reshape(rows, N)
+                assert np.all(leaf[step % rows] == loop.max_priority ** 0.6) and len(np.unique(leaf)) > N
+            if step >= 1:
+                u = rng.rand(40)
+                beta = 0.4 + 0.6 * step / steps
+                i1, w1 = vec.sample(u, beta)
+                i2, w2 = loop.sample(u, beta)
+                i3, w3 = tree_sample_model(s, m, loop.size, loop.tree_cap, u, beta)
+                assert np.array_equal(i1, i2) and np.array_equal(w1, w2) and np.array_equal(i3, i2) and np.array_equal(w3, w2)
+                td = rng.randn(40).astype(np.float32) * 3
+                i1[5:9] = i1[0]                              # a repeated index: the last occurrence's priority stays
+                vec.update(i1, td, 1e-6); loop.update_priorities(i1, td, 1e-6)
+                assert vec.sum[vec.tree_cap + i1[0]] == float(np.float32(abs(td[8])) + np.float32(1e-6)) ** 0.6 or i1[0] in i1[9:]
+            s, m = loop.trees()
+            assert np.array_equal(vec.sum[1:], s[1:]) and np.array_equal(vec.min[1:], m[1:]) and vec.max_priority == loop.max_priority
+            assert vec.size == loop.size == min(step + 1, rows) * N
     # masses at and next to the boundaries between leaves (a total of 8: u = mass / 8 is exact): the walk goes right at equality, as `left > mass` says
     t = SegmentTree(8, lambda a, b: a + b, 0.0)
     for i, x in enumerate([1.0, 2.0, 0.5, 0.25, 4.25]):

@@ -65,28 +65,44 @@ def test_sac_losses_gradient_matches_the_float64_model(W, A, ent_coef):
     assert want[ls_head] == 0 and want[ls_head + 1] == 0       # the clipped log_std heads get no gradient
 
 
-def test_torch_adam_polyak_matches_the_float64_tf_model():
+def _adam_polyak_against_the_model(warm):
+    """One case of test_torch_adam_polyak_matches_the_float64_tf_model: ``warm`` torch steps before the compared ones."""
     from rl_baselines.sac import SACNets, adam_polyak
     W, A = 3, 3
     torch.manual_seed(0)
     nets = SACNets(W, A)
-    arena0, target0 = nets.arena.detach().clone().numpy(), nets.target.clone().numpy()
     m, v = torch.zeros_like(nets.arena), torch.zeros_like(nets.arena)
     beta_power = torch.tensor([0.9, 0.999], dtype=torch.float32)
     g = torch.Generator().manual_seed(1)
+    for _ in range(warm):
+        adam_polyak(nets, torch.randn(nets.arena.numel(), generator=g), m, v, beta_power, 3e-4, 0.005, polyak=True)
+    arena0, target0 = nets.arena.detach().clone().numpy(), nets.target.clone().numpy()
+    m0, v0 = m.clone().numpy(), v.clone().numpy()
+    assert (np.abs(m0).max() > 0) == (warm > 0)
     grads = [torch.randn(nets.arena.numel(), generator=g) * (0.1 + k % 7) for k in range(100)]
     for k, gr in enumerate(grads):
         adam_polyak(nets, gr, m, v, beta_power, 3e-4, 0.005, polyak=True)
-    w, tg, mm, vv = adam_polyak_model(arena0, target0, [x.numpy() for x in grads], W, A, 3e-4, 0.005)
+    w, tg, mm, vv = adam_polyak_model(arena0, target0, [x.numpy() for x in grads], W, A, 3e-4, 0.005, m=m0, v=v0, steps=warm)
     scale = 3e-4 * 100
     assert np.abs(nets.arena.detach().numpy() - w).max() < 1e-4 * scale
     assert np.abs(nets.target.numpy() - tg).max() < 1e-4 * scale
     np.testing.assert_allclose(m.numpy(), mm, rtol=1e-4, atol=1e-6)
     np.testing.assert_allclose(v.numpy(), vv, rtol=1e-4, atol=1e-6)
-    assert np.allclose(beta_power.numpy(), [0.9 ** 101, 0.999 ** 101], rtol=1e-5)
+    assert np.allclose(beta_power.numpy(), [0.9 ** (warm + 101), 0.999 ** (warm + 101)], rtol=1e-5)
+    if warm:                                                   # the step count matters: the model one step off misses the first update
+        w1, _, _, _ = adam_polyak_model(arena0, target0, [grads[0].numpy()], W, A, 3e-4, 0.005, m=m0, v=v0, steps=warm)
+        w_off, _, _, _ = adam_polyak_model(arena0, target0, [grads[0].numpy()], W, A, 3e-4, 0.005, m=m0, v=v0, steps=warm - 1)
+        assert np.abs(w_off - w1).max() > 100 * np.abs(w1).max() * 2.0 ** -24
     before = nets.target.clone()
     adam_polyak(nets, grads[0], m, v, beta_power, 3e-4, 0.005, polyak=False)
     assert torch.equal(nets.target, before)
+
+
+def test_torch_adam_polyak_matches_the_float64_tf_model():
+    """100 steps of the torch statement against the float64 model, from zero slots and from the slots, beta powers and target that 37
+    earlier steps left (the model told only the slots and the step count)."""
+    for warm in (0, 37):
+        _adam_polyak_against_the_model(warm)
 
 
 def test_cadence():
